@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — LZ4 block compress+decompress throughput on B200 (BASELINE.json metric).
+"""bench.py — LZ4 block compress+decompress throughput on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA path through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference arm: CPU path on host cores
@@ -38,7 +38,7 @@ sys.path.insert(0, ROOT)
 BLOCK = 65536
 NBLOCKS_DEFAULT = 16384
 FIXTURE = "compression_66k_JSON.txt"
-METRIC = "LZ4 block MiB/s (compress+decompress) at 1/2/4/8 B200 vs CPU; % HBM peak"
+METRIC = "LZ4 block MiB/s (compress+decompress) at 1/2/4/8 H100 vs CPU; % HBM peak"
 
 
 def measured_peaks():
@@ -48,11 +48,11 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe).  NVML in-process at
+    """SM clock and throttle reasons sampled DURING the timed region.  NVML in-process at
     ~2 ms intervals (the timed region of the default run lasts ~0.25 s, too short for an `nvidia-smi -lms` loop to
     deliver samples); falls back to the nvidia-smi loop when pynvml is unavailable."""
 
@@ -155,27 +155,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "source": "nvidia-smi"}
 
 
-def ncu_traffic(kernel: str):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of `kernel` — the name the launcher reported
-    for this run (lz4b200_ctx_last_kernel) — from the committed ncu --set full summaries of this workload
-    (profiles/r2_ncu_summary.json, then r1), or None when that exact kernel has no capture: a profile is never
-    attributed to a kernel it was not taken from."""
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    norm = lambda n: n.replace("void ", "").split("(")[0].replace("lz4b200::", "").replace("(int)", "").replace("false", "0").replace("true", "1").replace(" ", "")
-    for f in ("r2_ncu_summary.json", "r1_ncu_summary.json"):
-        try:
-            for e in json.load(open(os.path.join(ROOT, "profiles", f))):
-                if norm(e.get("kernel", "")) == norm(kernel):
-                    tot = 0.0
-                    for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                        v, u = e[k].split()
-                        tot += float(v) * unit[u]
-                    return tot, f
-        except Exception:                                       # noqa: BLE001
-            pass
-    return None, None
-
-
 def build_workload(nblocks: int, rank: int):
     from lz4_flex_b200 import corpus
     total = nblocks * BLOCK
@@ -223,7 +202,7 @@ def cpu_arm(data: np.ndarray, nblocks: int, threads: int, repeats: int):
     key = ("bufs", nblocks, threads)
     if key not in _POOLS:
         # every buffer the workers stream through is first touched BY the workers (pool.copy), so its pages spread over the
-        # host's NUMA nodes instead of all sitting on the node of this thread (measured: 9.5 vs 35 GiB/s decompress)
+        # host's NUMA nodes instead of all sitting on the node of this thread
         comp = np.empty(nblocks * slot, dtype=np.uint8)
         back = np.empty(nblocks * BLOCK, dtype=np.uint8)
         src = np.empty(nblocks * BLOCK, dtype=np.uint8)
@@ -250,8 +229,8 @@ def cpu_arm(data: np.ndarray, nblocks: int, threads: int, repeats: int):
 
 def cpu_arm_fresh_process(nblocks: int):
     """The all-thread CPU baseline of the bench line, taken in a FRESH process (`bench.py --impl reference`): the same
-    thing the driver's reference arm runs.  Measured in-process after the GPU phases (CUDA context, pinned buffers, an
-    affinity binding undone) the same pool gave 10 GiB/s compress on a box where the fresh process gives 88 GiB/s."""
+    thing `--impl reference` runs.  Measured in-process after the GPU phases (CUDA context, pinned buffers, an affinity
+    binding undone) the same pool is several times slower than in a fresh process."""
     import subprocess
     try:
         r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "reference", "--steps", "3", "--warmup", "1",
@@ -414,6 +393,8 @@ def run_ours(args):
     t_end.record()
     torch.cuda.synchronize()
     k1_name, k2_name = _last_kernel(ctx, 0), _last_kernel(ctx, 1)       # what the launcher picked for the timed batches
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, enc, dec, d_comp, d_back, slot)
     if world > 1:
         dist.barrier()
     clocks = sampler.stop() if rank == 0 else None
@@ -581,9 +562,8 @@ def run_ours(args):
             raise err[0]
 
     best_chunks, e2e_s, e2e_how = 1, e2e_serial_s, "one call each, back to back"
-    # measured on B200 (profiles/r2_e2e_callers.txt): serial 48.6 ms; pipelined x2/x4/x8 51.6 / 54.3 / 66.7; pooled (8,2,1) /
-    # (8,3,2) / (16,3,2) / (16,4,2) 63.9 / 59.9 / 64.7 / 63.8 — the encoder's persistent CTAs leave the decoder no warp slots,
-    # so overlapping the two calls only adds per-call tails.  Two probes stay so that the record shows the comparison was made.
+    # The encoder's persistent CTAs leave the decoder no warp slots, so overlapping the two calls tends to add per-call tails
+    # rather than hide copies.  Two probes stay so that the record shows the comparison against one call at a time.
     cands = [("pipelined", (2,)), ("pooled", (8, 3, 2))]
     if os.environ.get("LZ4B200_E2E_POOL"):               # tuning aid: "chunks,compress_threads,decompress_threads;..."
         cands = [("pooled", tuple(int(v) for v in c.split(","))) for c in os.environ["LZ4B200_E2E_POOL"].split(";")]
@@ -645,8 +625,8 @@ def run_ours(args):
     stream_rec, stream_failed = None, None
     if nb >= 4096:
         K = 4 * e2e_steps                               # 20 batches by default: fill + drain add one tick to K
-        # (free-running variants — no join per tick, one or two compress threads — were slower at N=1, 39.8-41.4 ms vs 37.6,
-        # and the two-compress-thread one once handed the decoder an incomplete buffer at N=8: not kept.)
+        # (free-running variants — no join per tick, one or two compress threads — are not kept: the two-compress-thread one
+        # could hand the decoder an incomplete buffer.)
         ts, stream_err = [], None
         for it in range(3):                                 # a failure on one rank must not leave the others in a collective
             h_back.numpy()[::4096] = 0
@@ -709,8 +689,6 @@ def run_ours(args):
             dist.destroy_process_group()
         return
 
-    k1_traffic, k1_src = ncu_traffic(k1_name)
-    k2_traffic, k2_src = ncu_traffic(k2_name)
     mib_rank = nb * BLOCK / 2**20
     ms_per_step = elapsed_ms / args.steps
     value = world * mib_rank / (ms_per_step / 1e3)
@@ -737,21 +715,15 @@ def run_ours(args):
         "data": f"{FIXTURE} tiled (deterministic corpus fixture, BASELINE config 2); inputs larger than L2",
         "config": {"workload": f"{nb} x 64 KiB JSON blocks per GPU (1 GiB), block format, compress+decompress, "
                                f"byte-identical to the oracle", "block_bytes": BLOCK, "blocks_per_gpu": nb,
-                   "l2_policy": "inputs (1 GiB in, 0.24 GiB compressed, 1 GiB out per step) larger than the 126 MB L2",
+                   "l2_policy": "inputs (1 GiB in, 0.24 GiB compressed, 1 GiB out per step) larger than the 50 MB L2",
                    "ratio": comp_bytes / (nb * BLOCK)},
         "compress_mibs": world * mib_rank / (t_c / 1e3), "decompress_mibs": world * mib_rank / (t_d / 1e3),
         "compress_ms": t_c, "decompress_ms": t_d,
-        # traffic = dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu --set full capture of
-        # the same workload (profiles/r1_ncu_summary.json; see ncu_traffic())
         "roofline": {"kernel": k1_name, "bound": "hbm", "achieved": ach_c, "peak": peak,
-                     "unit": "GB/s", "frac": ach_c / peak, "traffic": k1_traffic if nb == NBLOCKS_DEFAULT else None,
-                     "traffic_source": f"profiles/{k1_src} (ncu --set full capture of this kernel on this workload)" if k1_src else None,
-                     "peak_source": peak_src,
+                     "unit": "GB/s", "frac": ach_c / peak, "traffic": None, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": alg_bytes},
         "roofline_decompress": {"kernel": k2_name, "bound": "hbm", "achieved": ach_d, "peak": peak,
-                                "unit": "GB/s", "frac": ach_d / peak,
-                                "traffic": k2_traffic if nb == NBLOCKS_DEFAULT else None,
-                                "traffic_source": f"profiles/{k2_src}" if k2_src else None, "peak_source": peak_src,
+                                "unit": "GB/s", "frac": ach_d / peak, "traffic": None, "peak_source": peak_src,
                                 "algorithmic_bytes_per_launch": alg_bytes},
         "cpu_baseline": None if cpu_all is None else {
             "value": cpu_all["roundtrip_mibs"], "unit": "MiB/s", "cores": cores, "threads": threads, "kind": "port",
@@ -782,6 +754,35 @@ def run_ours(args):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE_BLOCKS = 64
+DUMP_SEED = 0
+
+
+def dump_outputs(out_dir: str, enc, dec, d_comp, d_back, slot: int):
+    """What the last timed step handed its caller, as .npy files that two builds can be compared by: per-block compressed
+    lengths, decompressed lengths and statuses of the whole batch, and the compressed and decompressed bytes of a fixed,
+    seeded sample of DUMP_SAMPLE_BLOCKS blocks (the full outputs are 1.25 GiB; the sample keeps the dump under 40 MB)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    nb = enc.nblocks
+    clen = enc.out_len.cpu().numpy().astype(np.int64)
+    pick = np.sort(np.random.default_rng(DUMP_SEED).choice(nb, size=min(DUMP_SAMPLE_BLOCKS, nb), replace=False))
+    idx = torch.from_numpy(pick).to(d_comp.device)
+    comp = d_comp.view(nb, slot)[idx].cpu().numpy()
+    back = d_back.view(nb, BLOCK)[idx].cpu().numpy()
+    arrays = {
+        "compressed_len": clen.astype(np.float64),
+        "compress_status": enc.status.cpu().numpy().astype(np.float64),
+        "decompressed_len": dec.out_len.cpu().numpy().astype(np.float64),
+        "decompress_status": dec.status.cpu().numpy().astype(np.float64),
+        "sample_blocks": pick.astype(np.float64),
+        "sample_compressed_bytes": np.concatenate([comp[i, :clen[b]] for i, b in enumerate(pick)]).astype(np.float32),
+        "sample_decompressed_bytes": back.reshape(-1).astype(np.float32),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def hdfs_range(lo: int, n: int) -> np.ndarray:
@@ -964,6 +965,7 @@ def main():
                     help="blocks = BASELINE config 2 (default); frame = config 4 sharded frame + NCCL gather")
     ap.add_argument("--frame-blocks", type=int, default=256, help="4 MiB blocks per GPU for the sharded-frame record")
     ap.add_argument("--no-frame", action="store_true", help="skip the sharded-frame record (tuning aid)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     if args.workload == "frame" and args.impl == "ours":
         run_frame(args)

@@ -1,9 +1,9 @@
 /*
- * lz4b200.h — C ABI of the B200-native LZ4 block codec (liblz4b200.so).
+ * lz4b200.h — C ABI of the H100-native (sm_90a) LZ4 block codec (liblz4b200.so).
  *
  * This is the drop-in boundary for lz4_flex's block path.  lz4_flex has no FFI of its own:
  * its boundary is the crate's public Rust API.  Every entry point below names the Rust item
- * (file:line under /root/reference) whose work it takes over; INTEGRATION.md shows the
+ * (file:line in the lz4_flex v0.12.0 source tree) whose work it takes over; INTEGRATION.md shows the
  * `extern "C"` block + safe wrappers a maintainer adds on the Rust side.
  *
  * Conventions
@@ -110,8 +110,8 @@ const char *lz4b200_ctx_last_kernel(const lz4b200_ctx *ctx, int which);
 size_t lz4b200_max_output_size(size_t input_len);
 
 /* ---- block API, one block, host pointers -------------------------------------------------
- * 1:1 replacements.  One call = one block = ONE serial parse chain on the GPU: a 64 KiB block costs >= 2.6 ms to
- * compress and ~1 ms to decompress however empty the machine is (a CPU core needs 40 us / 15 us) — these calls are
+ * 1:1 replacements.  One call = one block = ONE serial parse chain on the GPU: a 64 KiB block costs milliseconds to
+ * compress and decompress however empty the machine is (a CPU core needs tens of microseconds) — these calls are
  * chain-latency-bound, not PCIe-bound.  They exist for drop-in completeness; throughput comes from the batch calls,
  * which run thousands of such chains at once (INTEGRATION.md section 2, "Which call"). */
 

@@ -1,4 +1,4 @@
-"""lz4_flex_b200 — a B200-native (sm_100a) LZ4 block codec behind lz4_flex's API surface.
+"""lz4_flex_b200 — an H100-native (sm_90a) LZ4 block codec behind lz4_flex's API surface.
 
 Layout mirrors the crate: `block` (compress*/decompress* free functions, error enums), `frame`
 (FrameEncoder/FrameDecoder/FrameInfo), and the crate-root re-exports of lib.rs:96-105.  Everything

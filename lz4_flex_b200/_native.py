@@ -1,6 +1,6 @@
 """Loader/builder of liblz4b200.so (the CUDA C-ABI library, include/lz4b200.h).
 
-The library is built IN-TREE with nvcc for sm_100a and loaded with ctypes.  There is no Python or
+The library is built in-tree with nvcc for sm_90a and loaded with ctypes.  There is no Python or
 CPU implementation behind these bindings: if the library is missing it is rebuilt, and if it cannot be
 loaded or no CUDA device exists, every call fails loudly.
 """
@@ -17,7 +17,7 @@ SO_PATH = os.environ.get("LZ4B200_SO_OVERRIDE") or os.path.join(_PKG, "liblz4b20
 HEADER = os.path.join(os.path.dirname(_PKG), "include", "lz4b200.h")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]
 
@@ -51,7 +51,7 @@ def build_ab(force: bool = False) -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """nvcc -gencode arch=compute_100a,code=sm_100a ... -> lz4_flex_b200/liblz4b200.so"""
+    """nvcc -gencode arch=compute_90a,code=sm_90a ... -> lz4_flex_b200/liblz4b200.so"""
     if os.environ.get("LZ4B200_SO_OVERRIDE"):
         return SO_PATH
     if not force and not _stale():

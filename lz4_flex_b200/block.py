@@ -1,8 +1,8 @@
-"""lz4_flex::block, B200 edition.
+"""lz4_flex::block, H100 edition.
 
 Same names, argument meaning and error behaviour as the crate's block API (reference
 src/block/compress.rs:588-692, src/block/decompress.rs:454-517, src/block/mod.rs:151-157); every call
-goes through the C ABI in include/lz4b200.h into the sm_100a kernels.  The single-block functions are
+goes through the C ABI in include/lz4b200.h into the sm_90a kernels.  The single-block functions are
 1:1 replacements and PCIe-bound by construction; `compress_batch` / `decompress_batch` (many independent
 blocks per launch) are the throughput path, and `DeviceBatch` is the device-pointer form bench.py times.
 """

@@ -1,4 +1,4 @@
-// lz4b200_api.cu — host runtime and C ABI (include/lz4b200.h) of the B200 LZ4 block codec.
+// lz4b200_api.cu — host runtime and C ABI (include/lz4b200.h) of the H100 (sm_90a) LZ4 block codec.
 //
 // Everything here is product code: contexts, launch plumbing, host<->device staging and the
 // frame container (header / BlockInfo / checksums), which is host-side bookkeeping around the
@@ -276,7 +276,7 @@ struct lz4b200_ctx {
     int enc_gtab_smem = 0;
     DevBuf<uint16_t> d_ttab16;                // K1-T tables
     DevBuf<uint32_t> d_gtag32;                // tagged global tables (lz4_compress_blocks_gtag)
-    int enc_gtag = 0;                         // LZ4B200_ENC_GTAG=71|62: tagged entries (measured slower: 19.4 vs 17.8 ms)
+    int enc_gtag = 0;                         // LZ4B200_ENC_GTAG=71|62: tagged entries (measured slower)
     int enc_gtag_ctas = 8;
     int enc_single_warp = 0;                  // LZ4B200_ENC_SINGLE_WARP=1: one warp searches and emits
     int dec_ctas_override = 0;                // LZ4B200_DEC_CTAS=n CTAs per SM
@@ -318,6 +318,17 @@ constexpr int kEnc32Warps = 2;     // 2 x 16 KiB tables per CTA
 #ifndef ENC16_PAIRS
 #define ENC16_PAIRS 3
 #endif
+// Global-table encoder CTAs per SM (7 matchers + 1 emitter each, 8 KiB of table per matcher).  On an H100 the tables
+// must share a 50 MB L2 with the streaming input and output: 3 CTAs (21 chains per SM, 23 MB of tables) with the register
+// budget of 3 CTAs (no spills) compress 1 GiB of 64 KiB JSON blocks 2.2x faster than filling all 64 warp slots with
+// 8 CTAs at 32 registers (61 MB of tables); 2, 4, 5 and 6 CTAs are slower too (DESIGN.md §6).
+#ifndef ENC_GTAB_CTAS
+#define ENC_GTAB_CTAS 3
+#endif
+constexpr int kGtabCtasPerSm = ENC_GTAB_CTAS;
+#define LZ4B200_STR2(x) #x
+#define LZ4B200_STR(x) LZ4B200_STR2(x)
+constexpr const char *kGtabKernelName = "lz4_compress_blocks_gtab<unsigned short, 7, 1, 0, " LZ4B200_STR(ENC_GTAB_CTAS) ">";
 constexpr int kEnc16Pairs = ENC16_PAIRS;   // split encoder: matcher+emitter pairs per CTA (named barriers: <= 3)
 constexpr int kEnc32Pairs = 2;
 
@@ -362,7 +373,8 @@ int pick_dec_group(const lz4b200_ctx *ctx, uint32_t nblocks)
     if (ctx->dec_group_override) return ctx->dec_group_override;
 #endif
     (void)ctx;
-    // measured on B200, 64 KiB JSON blocks: 16 384 blocks -> G=8 4.2 ms, G=16 4.5 ms, G=32 5.8 ms (DESIGN.md)
+    // narrower groups win on large batches of 64 KiB JSON blocks (fewer warp-instructions per sequence); whole warps win
+    // when there are too few blocks to fill the GPU
     if (nblocks >= 12288) return 8;
     return nblocks >= 4096 ? 16 : 32;
 }
@@ -496,7 +508,7 @@ static bool launch_compress_variant(lz4b200_ctx *ctx, const BatchArgs &a, uint32
 
 // K1 launcher.  Blocks <= 64 KiB: u16 tables; larger: u32 tables; unknown mix (max_in_len == 0): both kernels run over
 // the same ticket space and each skips the other's blocks.
-//   many small blocks (> 24 per SM, no dictionary)  -> global tables (56 chains per SM; half-warp matchers: 96+)
+//   many small blocks (> 24 per SM, no dictionary)  -> global tables (21 chains per SM; lane-group matchers: more)
 //   fewer / dictionary                              -> shared-memory tables, matcher + emitter pairs
 //   blocks > 64 KiB without dictionary              -> one chain per CTA over the TMA-fed ring when enabled
 lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t max_in_len, cudaStream_t s,
@@ -522,7 +534,7 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
         if (!a.dict_len && a.nblocks > (uint32_t)ctx->sm_count * 24u) {
             // u16 entries: CTAs per SM x chains per CTA tables of 4096, one region per concurrently running launch
             const int g16_m = (ctx->enc_g16 % 100) / 10, g16_g = ctx->enc_g16 >= 800 ? 8 : 16;
-            const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : 8u * 7u);   // enc_nib: A/B build only
+            const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : ctx->enc_nib ? 8u * 7u : (size_t)kGtabCtasPerSm * 7u);   // enc_nib: A/B build only
             const size_t region = (size_t)ctx->sm_count * chains_per_sm * 4096u;
             if (!ctx->check(ctx->d_gtab16.reserve(region * 9u), "gtab")) return LZ4B200_CUDA_ERROR;
             uint16_t *gt = ctx->d_gtab16.p + table_slot(ctx, tickets) * region;
@@ -551,9 +563,9 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
                 else if (m == 7) { lz4_compress_blocks_gtabg<16, 7, 1><<<grid, 256, 0, s>>>(a, tickets + 2, gt); ctx->last_kernel[0] = "lz4_compress_blocks_gtabg<16, 7, 1>"; }
                 else { lz4_compress_blocks_gtabg<16, 6, 2><<<grid, 256, 0, s>>>(a, tickets + 2, gt); ctx->last_kernel[0] = "lz4_compress_blocks_gtabg<16, 6, 2>"; }
             } else {
-                const uint32_t grid = std::min<uint32_t>((a.nblocks + 6) / 7, (uint32_t)ctx->sm_count * 8u);
-                lz4_compress_blocks_gtab<uint16_t, 7, 1, 0><<<grid, 256, 0, s>>>(a, tickets + 2, gt);
-                ctx->last_kernel[0] = "lz4_compress_blocks_gtab<unsigned short, 7, 1, 0>";
+                const uint32_t grid = std::min<uint32_t>((a.nblocks + 6) / 7, (uint32_t)ctx->sm_count * kGtabCtasPerSm);
+                lz4_compress_blocks_gtab<uint16_t, 7, 1, 0, kGtabCtasPerSm><<<grid, 256, 0, s>>>(a, tickets + 2, gt);
+                ctx->last_kernel[0] = kGtabKernelName;
             }
         } else {
             ctx->last_kernel[0] = "lz4_compress_blocks_split<unsigned short, 3, 0>";
@@ -871,19 +883,19 @@ lz4b200_status lz4b200_decompress_batch_device_with_dict(lz4b200_ctx *ctx, const
 namespace {
 
 constexpr int kMaxLanes = 8;
-// Lanes in flight.  A compress chunk occupies its lane for H2D + kernel (one block's serial chain, ~5 ms) + the
-// size read-back + D2H, ~10 ms in all, so three lanes cap the call at ~3.5 ms per 128 MiB chunk whatever the
-// kernel does (measured 30 ms per GiB); eight lanes leave the kernel / PCIe as the bound (26.8 ms).  LZ4B200_LANES overrides.
+// Lanes in flight.  A compress chunk occupies its lane for H2D + kernel (at least one block's serial chain, several ms)
+// + the size read-back + D2H, so a few lanes cap the call whatever the kernel does; eight lanes leave the kernel / PCIe as
+// the bound.  LZ4B200_LANES overrides.
 static int lanes_in_use()
 {
     static const int v = [] { const char *e = getenv("LZ4B200_LANES"); int k = e ? atoi(e) : 8; return k < 1 ? 1 : (k > kMaxLanes ? kMaxLanes : k); }();
     return v;
 }
-// decompress: a chunk's kernel lasts at least one block's serial chain (~1 ms for 64 KiB of JSON) however few blocks
-// it holds, so chunks must be big enough for that to hide behind the chunk's own D2H copy (2.3 ms per 128 MiB)
+// decompress: a chunk's kernel lasts at least one block's serial chain (about a millisecond for 64 KiB of JSON) however
+// few blocks it holds, so chunks must be big enough for that to hide behind the chunk's own D2H copy
 constexpr uint64_t kChunkBytesDefault = 128ull << 20;
-// compress: a 64 KiB block is one ~5 ms serial chain whatever the batch size, so a chunk must hold enough blocks
-// (2048 = 58 % of the resident warps) for two chunks in flight to fill the GPU
+// compress: a 64 KiB block is one serial chain of several ms whatever the batch size, so a chunk must hold enough blocks
+// (2048) for two chunks in flight to fill the GPU
 constexpr uint64_t kCompressChunkBytesDefault = 128ull << 20;
 
 uint64_t env_mib(const char *name, uint64_t dflt)         // tuning aid: chunk sizes in MiB
@@ -997,8 +1009,8 @@ static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *
         Chunk c{b, b, ~0ull, 0, 0, 0};
         uint64_t bytes = 0;
         // ramp: the first chunks are small (32, 64, ... MiB) so the first kernel starts after a short copy.  (Shrinking the
-        // LAST chunks as well — so that less work waits behind the last copy — was measured: 27.9 vs 26.5 ms per call; the
-        // extra chunks' read-back / pack / D2H round trips cost more than the shorter tail saves.)
+        // LAST chunks as well — so that less work waits behind the last copy — was measured slower: the extra chunks'
+        // read-back / pack / D2H round trips cost more than the shorter tail saves.)
         const uint64_t limit = std::min<uint64_t>(kCompressChunkBytes, (32ull << 20) << std::min<size_t>(chunks.size(), 8));
         while (c.b1 < nb && (c.b1 == c.b0 || bytes + in_len[c.b1] <= limit)) {
             const uint32_t k = c.b1++;

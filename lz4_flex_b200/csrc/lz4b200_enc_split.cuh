@@ -27,7 +27,7 @@
 #define ENC_GTAB_L1 0   // 1: global-table reads may hit L1 (same-SM coherent); 0: L2 only
 #endif
 #ifndef ENC_FIRST_WIDTH
-#define ENC_FIRST_WIDTH 32  // lanes probing in the first round of a sequence (8: 22.4 vs 20.6 ms — the extra round costs more than the traffic it saves)
+#define ENC_FIRST_WIDTH 32  // lanes probing in the first round of a sequence (8 was slower: the extra round costs more than the traffic it saves)
 #endif
 #ifndef ENC_FASTW
 #define ENC_FASTW 1     // 1: settle slot collisions of the first <= 4 probes with shuffles instead of match.any
@@ -39,7 +39,7 @@
 #define ENC_EMIT_SLEEP_NS 1000   // emitter back-off while its queue is empty (0: spin)
 #endif
 #ifndef ENC_WINDOW
-#define ENC_WINDOW 0   // 1: first probe batch reads a cp.async-filled shared-memory ring (measured: 20.6 vs 20.1 ms without)
+#define ENC_WINDOW 0   // 1: first probe batch reads a cp.async-filled shared-memory ring (measured slightly slower)
 #endif
 
 namespace lz4b200 {
@@ -74,8 +74,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
     } while (!done);
 }
 // Producer-side wait for a free ring half.  One emitter serves 7 matchers, so a matcher finds its half still unread
-// every few batches; spinning there cost 2.46 G of the kernel's 16.6 G warp-instructions (YIELD / try_wait / BRA, 819 M
-// iterations — ncu source page of profiles/r2_ncu_summary.json's capture) in a kernel that is bound by instruction issue.
+// every few batches; spinning there cost about a seventh of the kernel's warp-instructions (YIELD / try_wait / BRA) in a
+// kernel that is bound by instruction issue.
 // One immediate probe (the common case: already free), then try_wait with a suspend hint + nanosleep.
 #ifndef ENC_PROD_SLEEP_NS
 #define ENC_PROD_SLEEP_NS 200   // 0: spin (round-1 behaviour)
@@ -235,14 +235,12 @@ struct InputWindow {
 // in global memory and is read/written through L2 (ld/st.global.cg): ~250 cycles instead of 29 per access, but no
 // shared memory per matcher, so the matchers per SM are bounded by warps and registers instead of by 8 KiB tables.
 // Global tables are accessed with an L2 evict_last policy (createpolicy is a constant: it folds into the access
-// descriptor): 66 MB of tables must stay resident in the 126 MB L2 while ~0.5 GB of input streams through it —
-// without the hint the tables are evicted and every probe becomes a DRAM read (27.6 GB read per GiB compressed).
-// Both measured on B200 (profiles/r2_sweep_gnib_v2.txt): the global-table kernels are bound by instruction issue (~0.8 G
-// warp-instructions per ms whatever the variant), and with 32 registers per thread the compiler re-derives a chain's table
-// pointer from blockIdx / threadIdx and rebuilds the createpolicy descriptor (5 uniform instructions) at every table access.
-//   ENC_TAB_OPAQUE = 1: the chain's table offset lives in one opaque 32-bit register            17.77 -> 17.45 ms
-//   ENC_POLICY_HOIST = 1: createpolicy may be hoisted (uniform registers)                 with opaque: 17.17 ms
-//   ENC_POLICY_HOIST = 2: u16 table accesses without the evict_last hint (the hint was neutral)  with opaque: 16.46 ms (dickens 37.35 -> 34.55)
+// descriptor): the tables (8 KiB per chain) should stay resident in L2 while the input streams through it.
+// With 32 registers per thread the compiler re-derives a chain's table pointer from blockIdx / threadIdx and rebuilds the
+// createpolicy descriptor (5 uniform instructions) at every table access, in kernels that are bound by instruction issue:
+//   ENC_TAB_OPAQUE = 1: the chain's table offset lives in one opaque 32-bit register (faster)
+//   ENC_POLICY_HOIST = 1: createpolicy may be hoisted (uniform registers)
+//   ENC_POLICY_HOIST = 2: u16 table accesses without the evict_last hint (fastest: the hint was neutral)
 #ifndef ENC_POLICY_HOIST
 #define ENC_POLICY_HOIST 2
 #endif
@@ -312,7 +310,7 @@ __device__ __forceinline__ void tab_fill16(uint4 *at, uint32_t f)
 // kTag (global u32 tables, blocks <= 64 KiB): an entry is (tag << 16) | position, tag = 16 bits hashed from the 4 bytes
 // at that position.  A probe fetches its candidate's bytes only when the tags agree — a tag mismatch proves the 4-byte
 // comparison of compress.rs:432-438 fails, so the parse is unchanged — which removes ~30 of the 32 speculative sector
-// reads of a batch (the 40 GB of DRAM traffic per GiB that profiles/r1_ncu_summary.json shows for the untagged kernel).
+// reads of a batch (most of the DRAM traffic of the untagged kernel).
 __device__ __forceinline__ uint32_t tag16(uint32_t v4) { return (v4 * 2246822519u) >> 16; }
 
 template <typename TabT, bool kGT = false, bool kTag = false, typename View = WordView>
@@ -540,8 +538,7 @@ __device__ __forceinline__ void match_block(const uint8_t *__restrict__ src, uin
 // ---------------------------------------------------------------------------------------------
 // Matcher with 4-bit tags in SHARED memory beside the global position table (lz4_compress_blocks_gnib).
 // What `gtab` pays for its 56 chains per SM is table and candidate traffic: every probe batch loads 32 table entries
-// and 32 candidates (3.8 G L2 sector requests, 41 GB of DRAM traffic per GiB — profiles/r2_l2_sectors_by_instruction.md)
-// although the sequential loop of compress.rs:373-439 stops at the first match, 2.4 probes in on JSON.  Here every
+// and 32 candidates although the sequential loop of compress.rs:373-439 stops at the first match, 2.4 probes in on JSON.  Here every
 // slot also has a 4-bit tag of the 4 bytes at its position, 2 KiB per chain in shared memory (8 x 7 chains = 112 KB per
 // SM).  A probe whose tag disagrees cannot pass the 4-byte comparison (compress.rs:432-438), so it touches neither the
 // table nor its candidate.  The tag-matching probes are verified TWO at a time in probe order and the search stops at
@@ -555,7 +552,7 @@ __device__ __forceinline__ void match_block(const uint8_t *__restrict__ src, uin
 // may own different nibbles of a word); kTagBits = 8 -> bytes, 4 KiB per chain, plain byte stores.  The chain's tag array
 // and its table are addressed through two opaque 32-bit values (a shared-memory address and a byte offset from the table
 // base): with 32-40 registers per thread the compiler otherwise re-derives both pointers from threadIdx / blockIdx in
-// every divergent block (~30 instructions each, profiles/r2_ncu_gnib.md).
+// every divergent block (~30 instructions each).
 template <int kTagBits> __device__ __forceinline__ uint32_t tagof(uint32_t v4) { return (v4 * 2246822519u) >> (32 - kTagBits); }
 
 __device__ __forceinline__ uint32_t opaque32(uint32_t v) { asm volatile("mov.b32 %0, %0;" : "+r"(v)); return v; }
@@ -1103,9 +1100,10 @@ __device__ __forceinline__ void matcher_loop(const BatchArgs &a, uint32_t *ticke
 // of the grid, held in L2 by an evict_last policy).  Shared-memory tables cap an SM at 24 matchers; global tables
 // cost ~250 cycles per access but none of the 228 KB, so with 32 registers per thread all 64 warps of an SM work:
 // e.g. 8 CTAs x (2 shared + 5 global matchers + 1 emitter).  Blocks are pulled from one ticket queue, so the faster
-// shared-memory matchers simply take more of them.
-template <typename TabT, int kM, int kE, int kS>
-__global__ void __launch_bounds__((kM + kE) * 32, 2048 / ((kM + kE) * 32))
+// shared-memory matchers simply take more of them.  kCtas: resident CTAs per SM the launch plans for (sets the
+// register budget); the default fills all 64 warp slots.
+template <typename TabT, int kM, int kE, int kS, int kCtas = 2048 / ((kM + kE) * 32)>
+__global__ void __launch_bounds__((kM + kE) * 32, kCtas)
 lz4_compress_blocks_gtab(BatchArgs a, uint32_t *tickets, TabT *gtab)
 {
     constexpr int kR = kM / kE;
@@ -1216,8 +1214,7 @@ lz4_compress_blocks_gtag(BatchArgs a, uint32_t *tickets, uint32_t *gtab)
 
 // =============================================================================================
 // Half-warp matchers (lz4_compress_blocks_gtab16): TWO chains per matcher warp, 16 lanes each.
-// The global-table kernel is bound by instruction issue (13.8 G warp-instructions per GiB at IPC 2.6 of 4 per SM,
-// profiles/r1_ncu_summary.json), not by HBM: a sequence costs ~230 matcher instructions whether its batch needed 1 probe
+// The global-table kernel is bound by instruction issue while its tables stay in L2, not by HBM: a sequence costs ~230 matcher instructions whether its batch needed 1 probe
 // or 32.  Here the same instruction stream serves two blocks at once: each half of a warp owns a block, a table and a
 // tuple ring, every warp-level primitive runs under the half's mask, and the halves stay in step because the compiler
 // reconverges them at the end of every loop (a half that found its match waits while the other finishes its extra

@@ -1,4 +1,4 @@
-// lz4b200_kernels.cuh — sm_100a device code of the LZ4 block codec.
+// lz4b200_kernels.cuh — sm_90a device code of the LZ4 block codec.
 //
 // K2  lz4_decompress_blocks (+ _linked, _conv)  : decompress_internal  (reference src/block/decompress.rs:201-449)
 // K1  lz4_compress_blocks (single warp per block; A/B fallback)     : compress_internal (src/block/compress.rs:318-489)
@@ -9,7 +9,7 @@
 // counter.  This is latency-bound byte shuffling — no tensor cores.  See DESIGN.md for the layout,
 // the per-kernel roofline and what each phase costs.
 #pragma once
-// Build-time variant switches (A/B-measured on B200, see DESIGN.md §experiments).
+// Build-time variant switches (A/B-measured, see DESIGN.md §experiments).
 // ENC_SPLIT=1: matcher warp + emitter warp per block (lz4_compress_blocks_split); 0: one warp does both (v1).
 #ifndef ENC_SPLIT
 #define ENC_SPLIT 1
@@ -386,7 +386,7 @@ __device__ __forceinline__ DecResult decode_block_simple(const uint8_t *__restri
     if (n == 0) { r.status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; return r; }   // decompress.rs:207-209
     const WordView view(src);
     uint32_t ip = 0, op = 0;
-    // measured on B200 (DESIGN.md): deferral pays for 8-lane groups (4 byte-steps per match), not for wider ones
+    // deferral pays for 8-lane groups (4 byte-steps per match), not for wider ones
     constexpr bool kDefer = DEC_DEFER && G <= 8;
     uint8_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0;                // pending match bytes of this lane
 #if DEC_DEFER8
@@ -659,9 +659,9 @@ lz4_decompress_blocks_linked(BatchArgs a)
     }
 }
 
-// Warps per CTA.  A batch whose warps are all resident at once (<= 32 one-warp CTAs per SM: 16 384 blocks at G=8 are 27.7
-// warps per SM) runs as ONE-warp CTAs: the block scheduler spreads them evenly over the SMs and a finished warp frees its
-// slot at once (measured: 4.17 vs 4.32 ms on JSON, 7.97 vs 8.36 ms on dickens; two warps per CTA = four).  Larger batches
+// Warps per CTA.  A batch whose warps are all resident at once (<= 32 one-warp CTAs per SM: 16 384 blocks at G=8 are 31.0
+// warps per SM on 132 SMs) runs as ONE-warp CTAs: the block scheduler spreads them evenly over the SMs and a finished warp
+// frees its slot at once (faster than two or four warps per CTA on JSON and dickens).  Larger batches
 // keep DEC_WARPS_PER_CTA warps per CTA (32 CTAs per SM would cap one-warp CTAs at half the warp slots).
 #ifndef DEC_WARPS_PER_CTA
 #define DEC_WARPS_PER_CTA 4
@@ -669,7 +669,7 @@ lz4_decompress_blocks_linked(BatchArgs a)
 constexpr int kDecWarpsPerCta = DEC_WARPS_PER_CTA;
 
 // kDict: the batch has an external dictionary (decompress_into_with_dict); a separate instantiation so that the
-// plain kernel's register allocation is untouched (with the dictionary live ptxas spills in the hot loop: 4.2 -> 7.0 ms).
+// plain kernel's register allocation is untouched (with the dictionary live ptxas spills in the hot loop).
 template <int G, int kBatched, bool kDict, int kW = kDecWarpsPerCta>
 __global__ void __launch_bounds__(kW * 32)
 lz4_decompress_blocks(BatchArgs a)

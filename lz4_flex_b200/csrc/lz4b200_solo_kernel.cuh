@@ -113,7 +113,7 @@ lz4_compress_blocks_solo(BatchArgs a, uint32_t *tickets)
 
 // =============================================================================================
 // K1-S2: the same idea with the WARP matcher.  The single-thread matcher above pays ~5 cycles per dependent instruction
-// with nobody to hide them (measured: ~870 cycles per probe step, 185 ms per 4 MiB block); the warp matcher of
+// with nobody to hide them (hundreds of cycles per probe step); the warp matcher of
 // lz4b200_enc_split.cuh evaluates 32 probes per batch and extends 32 bytes per round, so the same dependent latency buys a
 // whole sequence.  match_block_view runs unchanged over a view that serves bytes from a shared-memory ring:
 //   * 64 KiB ring (power of two: index = x & 0xffff), 32 slots of 2 KiB, filled by TMA bulk copies issued six chunks

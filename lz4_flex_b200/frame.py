@@ -1,4 +1,4 @@
-"""lz4_flex::frame, B200 edition (encoder: independent-block mode; decoder: independent and linked blocks).
+"""lz4_flex::frame, H100 edition (encoder: independent-block mode; decoder: independent and linked blocks).
 
 FrameInfo / BlockSize / BlockMode / FrameEncoder / FrameDecoder with the reference's names and behaviour
 (src/frame/header.rs:39-192, src/frame/compress.rs:62-438, src/frame/decompress.rs:48-422).  The container

@@ -25,7 +25,7 @@
  * from two independent restatements agreeing (this file and the surveyor's), not from
  * lz4_flex itself.
  *
- * What follows what (reference file:line, relative to /root/reference):
+ * What follows what (reference file:line, relative to the lz4_flex v0.12.0 source tree):
  *   slot4()/slot5()          src/block/hashtable.rs:19-21, 27-34, 77-83, 121-127
  *   lz4o_max_output_size()   src/block/compress.rs:588-590
  *   encode_* (core parse)    src/block/compress.rs:318-489  (helpers :65-96, :156-247, :272-287)

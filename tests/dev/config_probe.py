@@ -1,4 +1,4 @@
-"""Development aid (run under gpurun): device-timed kernels for BASELINE configs 3 and 5 (not the bench metric).
+"""Development aid (run on a GPU): device-timed kernels for BASELINE configs 3 and 5 (not the bench metric).
 config 3: decompress-only, dickens.txt tiled to 1 GiB of 64 KiB blocks (oracle-compressed).
 config 5: 64 KiB all-zero blocks and incompressible blocks interleaved, zero fraction sweep."""
 import os, sys, time

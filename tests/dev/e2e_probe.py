@@ -1,4 +1,4 @@
-"""Development aid (run under gpurun): host-batch call timings for chunk-size / overlap tuning."""
+"""Development aid (run on a GPU): host-batch call timings for chunk-size / overlap tuning."""
 import os, sys, time, threading, queue
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import numpy as np, torch

@@ -1,4 +1,4 @@
-"""Ad-hoc GPU parity sweep (run under gpurun during development); the real tests are test_gpu_*.py."""
+"""Ad-hoc GPU parity sweep (run on a GPU during development); the real tests are test_gpu_*.py."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import numpy as np

@@ -1,4 +1,4 @@
-"""Dev sweep (gpurun): K1-T / K2-T launch shapes vs the warp-cooperative kernels on config 2 (and 3).
+"""Dev sweep (on a GPU): K1-T / K2-T launch shapes vs the warp-cooperative kernels on config 2 (and 3).
 Usage: python tests/dev/thread_sweep.py [nblocks] ; prints one line per shape: compress ms, decompress ms, parity."""
 import hashlib, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))

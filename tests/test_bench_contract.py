@@ -40,16 +40,6 @@ def test_reference_arm_is_silent_on_other_ranks():
     assert r.returncode == 0 and r.stdout.strip() == ""
 
 
-def test_ncu_traffic_lookup_is_by_exact_kernel():
-    sys.path.insert(0, ROOT)
-    import bench
-    got, src = bench.ncu_traffic("lz4_compress_blocks_gtab<unsigned short, 7, 1, 0>")
-    assert src == "r2_ncu_summary.json" and 3.0e10 < got < 6.0e10           # dram read + write of the committed capture
-    got2, src2 = bench.ncu_traffic("lz4_decompress_blocks<8, 0, 0, 1>")
-    assert src2 == "r2_ncu_summary.json" and 2.0e9 < got2 < 5.0e9
-    assert bench.ncu_traffic("lz4_compress_blocks_gtabg<8, 7, 1>") == (None, None)   # no capture of that kernel: no number
-
-
 def test_workload_is_the_tiled_fixture():
     sys.path.insert(0, ROOT)
     import bench

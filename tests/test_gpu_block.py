@@ -1,5 +1,5 @@
 """GPU parity tests of the block path: every call goes through the C ABI (include/lz4b200.h) into the
-sm_100a kernels and is compared with the CPU oracle — bit-exact for compressed bytes, decoded bytes, error
+sm_90a kernels and is compared with the CPU oracle — bit-exact for compressed bytes, decoded bytes, error
 codes and OutputTooSmall fields.  Structure follows the reference's tests/tests.rs."""
 import hashlib
 import json
