@@ -259,6 +259,7 @@ struct lz4b200_ctx {
     uint32_t *d_tickets = nullptr;            // 3 x {next, retired}
     int dec_ctas_per_sm = 0;
     int enc16s_ctas_per_sm = 0, enc32s_ctas_per_sm = 0;   // split (matcher+emitter) encoder
+    int enc_gtab_ctas_per_sm = 0;             // global-table encoder (must reach ENC_GTAB_CTAS)
     int high_priority = 0;                    // lz4b200_ctx_set_priority(ctx, 1): pipeline streams get the highest priority
     DevBuf<uint16_t> d_gtab16;                // global u16 tables (lz4_compress_blocks_gtab / _gtab16)
     const uint32_t *pipe_tickets = nullptr;  // base of the host pipeline's ticket blocks (selects a table region)
@@ -273,7 +274,6 @@ struct lz4b200_ctx {
 #ifdef LZ4B200_AB_VARIANTS
     int enc16_ctas_per_sm = 0, enc32_ctas_per_sm = 0;
     int enc_gtab = 71;                        // LZ4B200_ENC_GTAB=10*matchers+emitters per CTA (62|71|44|151)
-    int enc_gtab_smem = 0;
     DevBuf<uint16_t> d_ttab16;                // K1-T tables
     DevBuf<uint32_t> d_gtag32;                // tagged global tables (lz4_compress_blocks_gtag)
     int enc_gtag = 0;                         // LZ4B200_ENC_GTAG=71|62: tagged entries (measured slower)
@@ -318,17 +318,33 @@ constexpr int kEnc32Warps = 2;     // 2 x 16 KiB tables per CTA
 #ifndef ENC16_PAIRS
 #define ENC16_PAIRS 3
 #endif
-// Global-table encoder CTAs per SM (7 matchers + 1 emitter each, 8 KiB of table per matcher).  On an H100 the tables
-// must share a 50 MB L2 with the streaming input and output: 3 CTAs (21 chains per SM, 23 MB of tables) with the register
-// budget of 3 CTAs (no spills) compress 1 GiB of 64 KiB JSON blocks 2.2x faster than filling all 64 warp slots with
-// 8 CTAs at 32 registers (61 MB of tables); 2, 4, 5 and 6 CTAs are slower too (DESIGN.md §6).
+// Shape of the global-table encoder lz4_compress_blocks_gtab<u16, M, E, SMEM, CTAS>: M matcher warps and E emitter warps
+// per CTA, CTAS CTAs per SM (which also sets the register budget).  The first SMEM matchers of a CTA keep their 8 KiB
+// table in shared memory, the other M - SMEM in global memory, where every SM's tables share the 50 MB L2 of an H100
+// with the streaming input and output.  The default keeps all 21 tables of an SM in shared memory (183 KB with the
+// queues): no table traffic reaches L2, and the 60 KB of L1 left beside them still caches the input.  On one H100 at
+// 400 W it compresses 1 GiB of 64 KiB JSON blocks in 25 % less time than the same shape with global tables; more chains
+// per SM with part of the tables in global memory, or a larger shared-memory carveout that shrinks L1 to 28 KB, are
+// slower (DESIGN.md §6).
+#ifndef ENC_GTAB_M
+#define ENC_GTAB_M 7
+#endif
+#ifndef ENC_GTAB_E
+#define ENC_GTAB_E 1
+#endif
+#ifndef ENC_GTAB_SMEM
+#define ENC_GTAB_SMEM 7
+#endif
 #ifndef ENC_GTAB_CTAS
 #define ENC_GTAB_CTAS 3
 #endif
-constexpr int kGtabCtasPerSm = ENC_GTAB_CTAS;
+constexpr int kGtabM = ENC_GTAB_M, kGtabE = ENC_GTAB_E, kGtabSmem = ENC_GTAB_SMEM, kGtabCtasPerSm = ENC_GTAB_CTAS;
+constexpr int kGtabSmemBytes = kGtabSmem * 4096 * (int)sizeof(uint16_t);
+static_assert(kGtabSmem >= 0 && kGtabSmem <= kGtabM, "ENC_GTAB_SMEM: at most ENC_GTAB_M shared-memory tables");
 #define LZ4B200_STR2(x) #x
 #define LZ4B200_STR(x) LZ4B200_STR2(x)
-constexpr const char *kGtabKernelName = "lz4_compress_blocks_gtab<unsigned short, 7, 1, 0, " LZ4B200_STR(ENC_GTAB_CTAS) ">";
+constexpr const char *kGtabKernelName = "lz4_compress_blocks_gtab<unsigned short, " LZ4B200_STR(ENC_GTAB_M) ", " LZ4B200_STR(ENC_GTAB_E)
+                                        ", " LZ4B200_STR(ENC_GTAB_SMEM) ", " LZ4B200_STR(ENC_GTAB_CTAS) ">";
 constexpr int kEnc16Pairs = ENC16_PAIRS;   // split encoder: matcher+emitter pairs per CTA (named barriers: <= 3)
 constexpr int kEnc32Pairs = 2;
 
@@ -471,21 +487,16 @@ static bool launch_compress_variant(lz4b200_ctx *ctx, const BatchArgs &a, uint32
             if (!ctx->check(cudaGetLastError(), "gtag launch")) *st = LZ4B200_CUDA_ERROR;
             return true;
         }
-        const int m = ctx->enc_gtab / 10, e = ctx->enc_gtab % 10, ks = ctx->enc_gtab_smem;
-        if (ctx->enc_gtab && (m != 7 || e != 1 || ks)) {                              // other global-table CTA shapes
-            const uint32_t want = (a.nblocks + m - 1) / m;
-            uint32_t grid = std::min<uint32_t>(want, (uint32_t)ctx->sm_count * (m == 15 ? 4u : 8u));
+        const int m = ctx->enc_gtab / 10, e = ctx->enc_gtab % 10;
+        if (ctx->enc_gtab && (m != 7 || e != 1)) {                                   // other global-table CTA shapes
+            const uint32_t grid = std::min<uint32_t>((a.nblocks + m - 1) / m, (uint32_t)ctx->sm_count * (m == 15 ? 4u : 8u));
             const size_t region = (size_t)ctx->sm_count * 8u * 28u * 4096u;
             if (!ctx->check(ctx->d_gtab16.reserve(region * 9u), "gtab")) { *st = LZ4B200_CUDA_ERROR; return true; }
             uint16_t *gt = ctx->d_gtab16.p + slot * region;
             if (m == 15) lz4_compress_blocks_gtab<uint16_t, 15, 1, 0><<<grid, 512, 0, s>>>(a, tickets + 2, gt);
             else if (m == 6 && e == 2) lz4_compress_blocks_gtab<uint16_t, 6, 2, 0><<<grid, 256, 0, s>>>(a, tickets + 2, gt);
             else if (m == 4 && e == 4) lz4_compress_blocks_gtab<uint16_t, 4, 4, 0><<<grid, 256, 0, s>>>(a, tickets + 2, gt);
-            else if (ks == 2) lz4_compress_blocks_gtab<uint16_t, 7, 1, 2><<<grid, 256, 2 * 8192, s>>>(a, tickets + 2, gt);
-            else if (ks == 3) {
-                grid = std::min<uint32_t>(want, (uint32_t)ctx->sm_count * 7u);
-                lz4_compress_blocks_gtab<uint16_t, 7, 1, 3><<<grid, 256, 3 * 8192, s>>>(a, tickets + 2, gt);
-            } else return false;
+            else return false;
             if (!ctx->check(cudaGetLastError(), "gtab launch")) *st = LZ4B200_CUDA_ERROR;
             return true;
         }
@@ -508,7 +519,8 @@ static bool launch_compress_variant(lz4b200_ctx *ctx, const BatchArgs &a, uint32
 
 // K1 launcher.  Blocks <= 64 KiB: u16 tables; larger: u32 tables; unknown mix (max_in_len == 0): both kernels run over
 // the same ticket space and each skips the other's blocks.
-//   many small blocks (> 24 per SM, no dictionary)  -> global tables (21 chains per SM; lane-group matchers: more)
+//   many small blocks (> 24 per SM, no dictionary)  -> gtab: 7 matchers per emitter, ENC_GTAB_* shape (21 chains per SM,
+//                                                      tables in shared memory; lane-group matchers: more, global tables)
 //   fewer / dictionary                              -> shared-memory tables, matcher + emitter pairs
 //   blocks > 64 KiB without dictionary              -> one chain per CTA over the TMA-fed ring when enabled
 lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t max_in_len, cudaStream_t s,
@@ -532,9 +544,10 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
     }
     {                                                       // u16 tables: every block with input (+ dictionary) <= 64 KiB
         if (!a.dict_len && a.nblocks > (uint32_t)ctx->sm_count * 24u) {
-            // u16 entries: CTAs per SM x chains per CTA tables of 4096, one region per concurrently running launch
+            // u16 entries: tables of 4096 for the CTAs per SM x chains per CTA that keep them in global memory, one region
+            // per concurrently running launch
             const int g16_m = (ctx->enc_g16 % 100) / 10, g16_g = ctx->enc_g16 >= 800 ? 8 : 16;
-            const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : ctx->enc_nib ? 8u * 7u : (size_t)kGtabCtasPerSm * 7u);   // enc_nib: A/B build only
+            const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : ctx->enc_nib ? 8u * 7u : (size_t)kGtabCtasPerSm * (kGtabM - kGtabSmem));   // enc_nib: A/B build only
             const size_t region = (size_t)ctx->sm_count * chains_per_sm * 4096u;
             if (!ctx->check(ctx->d_gtab16.reserve(region * 9u), "gtab")) return LZ4B200_CUDA_ERROR;
             uint16_t *gt = ctx->d_gtab16.p + table_slot(ctx, tickets) * region;
@@ -563,8 +576,9 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
                 else if (m == 7) { lz4_compress_blocks_gtabg<16, 7, 1><<<grid, 256, 0, s>>>(a, tickets + 2, gt); ctx->last_kernel[0] = "lz4_compress_blocks_gtabg<16, 7, 1>"; }
                 else { lz4_compress_blocks_gtabg<16, 6, 2><<<grid, 256, 0, s>>>(a, tickets + 2, gt); ctx->last_kernel[0] = "lz4_compress_blocks_gtabg<16, 6, 2>"; }
             } else {
-                const uint32_t grid = std::min<uint32_t>((a.nblocks + 6) / 7, (uint32_t)ctx->sm_count * kGtabCtasPerSm);
-                lz4_compress_blocks_gtab<uint16_t, 7, 1, 0, kGtabCtasPerSm><<<grid, 256, 0, s>>>(a, tickets + 2, gt);
+                const uint32_t grid = std::min<uint32_t>((a.nblocks + kGtabM - 1) / kGtabM, (uint32_t)ctx->sm_count * kGtabCtasPerSm);
+                lz4_compress_blocks_gtab<uint16_t, kGtabM, kGtabE, kGtabSmem, kGtabCtasPerSm>
+                    <<<grid, (kGtabM + kGtabE) * 32, kGtabSmemBytes, s>>>(a, tickets + 2, gt);
                 ctx->last_kernel[0] = kGtabKernelName;
             }
         } else {
@@ -666,6 +680,25 @@ lz4b200_status lz4b200_ctx_create(int device, lz4b200_ctx **out)
                                              (int)kSolo2SmemBytes), "solo2 smem") &&
              ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->enc_solo2_ctas_per_sm, lz4_compress_blocks_solo2, 64,
                                                                       kSolo2SmemBytes), "occupancy solo2");
+        // The global-table encoder's register budget and table region assume ENC_GTAB_CTAS resident CTAs per SM.  Its
+        // carveout is the least shared memory those CTAs need (the driver rounds up to the next supported size): the rest
+        // of the SM's 256 KB stays L1, which caches the input bytes every probe and extension reads.
+        auto *gtab = lz4_compress_blocks_gtab<uint16_t, kGtabM, kGtabE, kGtabSmem, kGtabCtasPerSm>;
+        cudaFuncAttributes fa{};
+        int smem_sm = 0, smem_reserved = 0;
+        ok = ok && ctx->check(cudaFuncGetAttributes(&fa, gtab), "gtab attributes") &&
+             ctx->check(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device), "smem per SM") &&
+             ctx->check(cudaDeviceGetAttribute(&smem_reserved, cudaDevAttrReservedSharedMemoryPerBlock, device), "reserved smem");
+        if (ok) {
+            const size_t need = (size_t)kGtabCtasPerSm * (fa.sharedSizeBytes + kGtabSmemBytes + smem_reserved);
+            const int carveout = (int)std::min<size_t>(100, (need * 100 + smem_sm - 1) / std::max(1, smem_sm));
+            ok = ctx->check(cudaFuncSetAttribute(gtab, cudaFuncAttributeMaxDynamicSharedMemorySize, kGtabSmemBytes), "gtab smem") &&
+                 ctx->check(cudaFuncSetAttribute(gtab, cudaFuncAttributePreferredSharedMemoryCarveout, carveout), "gtab carveout") &&
+                 ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->enc_gtab_ctas_per_sm, gtab, (kGtabM + kGtabE) * 32,
+                                                                          kGtabSmemBytes), "occupancy gtab");
+            if (getenv("LZ4B200_DEBUG"))
+                fprintf(stderr, "lz4b200: %s: %zu bytes of shared memory per SM, carveout %d %%\n", kGtabKernelName, need, carveout);
+        }
         ctx->enc_solo_small_max = (uint32_t)(ctx->sm_count * std::max(1, ctx->enc_solo2_ctas_per_sm));
     }
 #ifdef LZ4B200_AB_VARIANTS
@@ -682,6 +715,11 @@ lz4b200_status lz4b200_ctx_create(int device, lz4b200_ctx **out)
                                                                       kSoloSmemBytes), "occupancy solo");
     }
 #endif
+    if (ok && ctx->enc_gtab_ctas_per_sm < kGtabCtasPerSm) {
+        ctx->last_error = std::string(kGtabKernelName) + ": " + std::to_string(ctx->enc_gtab_ctas_per_sm) + " resident CTAs per SM, " +
+                          std::to_string(kGtabCtasPerSm) + " planned";
+        ok = false;
+    }
     if (!ok || ctx->dec_ctas_per_sm < 1 || ctx->enc16s_ctas_per_sm < 1 || ctx->enc32s_ctas_per_sm < 1) {
         fprintf(stderr, "lz4b200: context creation failed: %s\n", ctx->last_error.c_str());
         lz4b200_ctx_destroy(ctx);
@@ -707,16 +745,15 @@ lz4b200_status lz4b200_ctx_create(int device, lz4b200_ctx **out)
     if (const char *g = getenv("LZ4B200_ENC_SOLO_SMALL_MAX")) ctx->enc_solo_small_max = (uint32_t)atoll(g);
     if (ctx->enc_solo2_ctas_per_sm < 1 && ctx->enc_solo == 2) ctx->enc_solo = 0;
     if (getenv("LZ4B200_DEBUG"))
-        fprintf(stderr, "lz4b200: SMs %d, CTAs/SM: dec %d, enc16-split %d (x%d pairs), enc32-split %d (x%d pairs), solo2 %d\n",
+        fprintf(stderr, "lz4b200: SMs %d, CTAs/SM: dec %d, enc16-split %d (x%d pairs), enc32-split %d (x%d pairs), solo2 %d, %s %d\n",
                 ctx->sm_count, ctx->dec_ctas_per_sm, ctx->enc16s_ctas_per_sm, kEnc16Pairs, ctx->enc32s_ctas_per_sm, kEnc32Pairs,
-                ctx->enc_solo2_ctas_per_sm);
+                ctx->enc_solo2_ctas_per_sm, kGtabKernelName, ctx->enc_gtab_ctas_per_sm);
 #ifdef LZ4B200_AB_VARIANTS
     if (ctx->enc_solo == 1 && ctx->enc_solo_ctas_per_sm < 1) ctx->enc_solo = 0;
     if (const char *g = getenv("LZ4B200_ENC_SINGLE_WARP")) ctx->enc_single_warp = atoi(g);
     if (const char *g = getenv("LZ4B200_ENC_GTAB")) ctx->enc_gtab = atoi(g);
     if (const char *g = getenv("LZ4B200_ENC_GTAG")) ctx->enc_gtag = atoi(g);
     if (const char *g = getenv("LZ4B200_ENC_GTAG_CTAS")) ctx->enc_gtag_ctas = std::max(1, std::min(8, atoi(g)));
-    if (const char *g = getenv("LZ4B200_ENC_GTAB_SMEM")) ctx->enc_gtab_smem = atoi(g);
     if (const char *g = getenv("LZ4B200_DEC_CTAS")) ctx->dec_ctas_override = atoi(g);
     if (const char *g = getenv("LZ4B200_DEC_BATCHED")) ctx->dec_batched = atoi(g);
     if (const char *g = getenv("LZ4B200_DEC_CONV")) ctx->dec_conv = atoi(g);

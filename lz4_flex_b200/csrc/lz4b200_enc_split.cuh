@@ -1,8 +1,9 @@
 // lz4b200_enc_split.cuh — K1 as a matcher/emitter warp pipeline (included by lz4b200_kernels.cuh).
 //
 // Two kernels share the code below: lz4_compress_blocks_split (one emitter per matcher, tables in shared memory,
-// 24 matchers per SM) and lz4_compress_blocks_gtab (7 matchers per emitter, tables in global memory served by
-// L2, 56 matchers per SM).  The launcher picks by batch size (DESIGN.md §4).
+// 24 matchers per SM) and lz4_compress_blocks_gtab (7 matchers per emitter, each table in shared memory or in global
+// memory served by L2; 21 matchers per SM by default, all with shared-memory tables).  The launcher picks by batch
+// size (DESIGN.md §4).
 //
 // compress_internal (reference src/block/compress.rs:318-489) does two things per sequence: it SEARCHES
 // (probe loop :373-439, backward/forward extension :272-287 / :156-216, the cur-2 re-insert :460-461) and it
@@ -1096,10 +1097,9 @@ __device__ __forceinline__ void matcher_loop(const BatchArgs &a, uint32_t *ticke
 }
 
 // Many-matcher variant: kM matcher warps + kE emitter warps per CTA (kM a multiple of kE).  The first kS matchers
-// of a CTA keep their table in shared memory; the others keep it in global memory (gtab, 4096 entries per matcher
-// of the grid, held in L2 by an evict_last policy).  Shared-memory tables cap an SM at 24 matchers; global tables
-// cost ~250 cycles per access but none of the 228 KB, so with 32 registers per thread all 64 warps of an SM work:
-// e.g. 8 CTAs x (2 shared + 5 global matchers + 1 emitter).  Blocks are pulled from one ticket queue, so the faster
+// of a CTA keep their table in shared memory (kS x 8 KiB of dynamic shared memory); the other kM - kS keep it in global
+// memory (gtab, 4096 entries for each of them, CTA after CTA).  Shared-memory tables cap an SM at 24 matchers; global tables cost
+// ~250 cycles per access but none of the 228 KB.  Blocks are pulled from one ticket queue, so the faster
 // shared-memory matchers simply take more of them.  kCtas: resident CTAs per SM the launch plans for (sets the
 // register budget); the default fills all 64 warp slots.
 template <typename TabT, int kM, int kE, int kS, int kCtas = 2048 / ((kM + kE) * 32)>
@@ -1126,12 +1126,13 @@ lz4_compress_blocks_gtab(BatchArgs a, uint32_t *tickets, TabT *gtab)
     if (kS > 0 && warp + 1u <= (uint32_t)kS)
         matcher_loop<TabT, false>(a, tickets, reinterpret_cast<TabT *>(smem_raw) + warp * 4096, pr, lane);
     else {
+        // tables of the kM - kS global matchers only, CTA after CTA (the launcher reserves exactly that many)
 #if ENC_TAB_OPAQUE
-        uint32_t toff = (blockIdx.x * kM + warp) * 4096u;          // opaque: not re-derived from blockIdx / threadIdx at every use
+        uint32_t toff = (blockIdx.x * (kM - kS) + warp - kS) * 4096u;   // opaque: not re-derived from blockIdx / threadIdx at every use
         asm volatile("mov.b32 %0, %0;" : "+r"(toff));
         matcher_loop<TabT, true>(a, tickets, gtab + toff, pr, lane);
 #else
-        matcher_loop<TabT, true>(a, tickets, gtab + ((size_t)blockIdx.x * kM + warp) * 4096, pr, lane);
+        matcher_loop<TabT, true>(a, tickets, gtab + ((size_t)blockIdx.x * (kM - kS) + warp - kS) * 4096, pr, lane);
 #endif
     }
     retire_warp(tickets, gridDim.x * kM);
