@@ -337,6 +337,22 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
  * blocks: their length).  The header's content_size is deliberately ignored (untrusted).  Host-side walk only. */
 lz4b200_status lz4b200_frame_decoded_bound(const uint8_t *in, size_t n, size_t *bound);
 
+/* lz4b200_frame_decompress_next for ONE frame whose bytes are in DEVICE memory, decoded into DEVICE memory.  For every
+ * input and every `cap` it returns what lz4b200_frame_decompress_next returns for the same bytes in host memory: status,
+ * consumed, written, block_status, err_expected, err_actual and the first `written` bytes of d_out (bytes of d_out past
+ * `written` are not written).  The header, the BlockInfo chain, the block checksums and the content checksum are
+ * processed on the GPU; only block descriptors (16 B per block) and per-group statuses cross PCIe.  d_in may have any
+ * alignment.  Work is enqueued on `stream` (NULL = legacy default stream, lz4b200_ctx_stream() = the context's own); the
+ * call synchronises that stream and returns with the result in d_out.  The result scalars are host pointers. */
+lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint8_t *d_out,
+                                                    size_t cap, size_t *consumed, size_t *written, int *block_status,
+                                                    uint64_t *err_expected, uint64_t *err_actual, void *stream);
+
+/* lz4b200_frame_decoded_bound for frames in device memory (every concatenated frame; content_size ignored); the walk runs
+ * on the GPU on `stream`, which the call synchronises. */
+lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
+                                                  void *stream);
+
 /* XXH32 (twox-hash XxHash32, Cargo.toml:51) — used for header/block/content checksums.
  * The streaming form backs FrameEncoder's running content hash (frame/compress.rs:141,320). */
 uint32_t lz4b200_xxh32(const uint8_t *data, size_t n, uint32_t seed);

@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
 #include "lz4b200_solo_kernel.cuh"
 #ifdef LZ4B200_AB_VARIANTS
@@ -146,58 +147,53 @@ __global__ void make_uniform_desc_kernel(uint64_t total_len, uint32_t block, uin
     }
 }
 
+// ---- device-resident frame decoder (lz4b200_frame_decompress_next_device) ----------------------------------------------
+
+// One thread walks the frame at `in` (fw::frame_walk, the same code the host path runs), resuming from *w and
+// recording at most max_blocks descriptors.
+__global__ void frame_walk_kernel(const uint8_t *in, uint64_t n, fw::FrameWalk *w, fw::FrameBlockDesc *out, uint32_t max_blocks)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0) fw::frame_walk(in, n, *w, out, max_blocks);
+}
+
+// Block checksums of the blocks the last walk launch recorded (frame indices first .. w->nblocks - 1), one thread per
+// block running the serial XXH32 over its payload; *bad receives the lowest index that fails.
+__global__ void __launch_bounds__(128) block_checksum_kernel(const uint8_t *in, const fw::FrameBlockDesc *desc,
+                                                             const fw::FrameWalk *w, uint64_t first, uint32_t *bad)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (!(w->flg & 0x10) || i >= w->nblocks - first) return;
+    if (!fw::block_checksum_ok(in, desc[i])) atomicMin(bad, (uint32_t)(first + i));
+}
+
+// The content checksum is one XXH32 chain over the whole output (frame/decompress.rs:323-331): thread 0 carries it
+// over each group's output as the group lands.  The other threads of the CTA only stage the bytes through shared
+// memory, so that the chain reads them at shared-memory latency rather than waiting on global memory stripe by stripe.
+constexpr uint32_t kHashStage = 16384;
+__global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *st, const uint8_t *p, uint64_t n)
+{
+    __shared__ uint8_t stage[kHashStage];
+    lz4b200_xxh32_state h;
+    if (threadIdx.x == 0) h = *st;
+    for (uint64_t o = 0; o < n; o += kHashStage) {
+        const uint32_t len = n - o < kHashStage ? (uint32_t)(n - o) : kHashStage;
+        for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) stage[i] = p[o + i];
+        __syncthreads();
+        if (threadIdx.x == 0) fw::xxh32_update(h, stage, len);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *st = h;
+}
+
 }  // namespace lz4b200
 
 // ---------------------------------------------------------------------------------------------
-// XXH32 (host) — header checksum byte, block and content checksums
+// host helpers
 // ---------------------------------------------------------------------------------------------
 namespace {
 
 inline uint32_t rd32(const uint8_t *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 inline void wr32(uint8_t *p, uint32_t v) { memcpy(p, &v, 4); }
-inline uint32_t rotl(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-
-constexpr uint32_t kP1 = 2654435761u, kP2 = 2246822519u, kP3 = 3266489917u, kP4 = 668265263u, kP5 = 374761393u;
-
-struct Xxh32 {
-    uint32_t acc[4];
-    uint8_t buf[16];
-    uint32_t fill = 0;
-    uint64_t total = 0;
-    uint32_t seed;
-    explicit Xxh32(uint32_t s = 0) : seed(s)
-    {
-        acc[0] = s + kP1 + kP2; acc[1] = s + kP2; acc[2] = s; acc[3] = s - kP1;
-    }
-    static uint32_t round(uint32_t a, uint32_t v) { return rotl(a + v * kP2, 13) * kP1; }
-    void stripe(const uint8_t *p)
-    {
-        for (int i = 0; i < 4; i++) acc[i] = round(acc[i], rd32(p + 4 * i));
-    }
-    void update(const uint8_t *p, size_t n)
-    {
-        total += n;
-        if (fill) {
-            size_t take = std::min<size_t>(16 - fill, n);
-            memcpy(buf + fill, p, take); fill += (uint32_t)take; p += take; n -= take;
-            if (fill < 16) return;
-            stripe(buf); fill = 0;
-        }
-        for (; n >= 16; p += 16, n -= 16) stripe(p);
-        if (n) { memcpy(buf, p, n); fill = (uint32_t)n; }
-    }
-    uint32_t digest() const
-    {
-        uint32_t h = total >= 16 ? rotl(acc[0], 1) + rotl(acc[1], 7) + rotl(acc[2], 12) + rotl(acc[3], 18)
-                                 : seed + kP5;
-        h += (uint32_t)total;
-        const uint8_t *p = buf, *e = buf + fill;
-        for (; p + 4 <= e; p += 4) h = rotl(h + rd32(p) * kP3, 17) * kP4;
-        for (; p < e; p++) h = rotl(h + (*p) * kP5, 11) * kP1;
-        h ^= h >> 15; h *= kP2; h ^= h >> 13; h *= kP3; h ^= h >> 16;
-        return h;
-    }
-};
 
 size_t block_size_bytes(int id)
 {
@@ -300,6 +296,12 @@ struct lz4b200_ctx {
     DevBuf<uint32_t> d_in_len, d_out_cap, d_out_len, d_info, d_seg_size, d_payload_len, d_link_first, d_stored_len, d_done;
     DevBuf<uint64_t> d_stored_off;
     DevBuf<int32_t> d_status;
+    // device-resident frame decoder: walk state, the block descriptors of one walk launch, the first block whose
+    // checksum fails, the running content hash
+    DevBuf<fw::FrameWalk> d_walk;
+    DevBuf<fw::FrameBlockDesc> d_desc;
+    DevBuf<uint32_t> d_bad;
+    DevBuf<lz4b200_xxh32_state> d_content;
 
     bool check(cudaError_t e, const char *what)
     {
@@ -788,6 +790,7 @@ void lz4b200_ctx_destroy(lz4b200_ctx *ctx)
     ctx->d_in_len.release(); ctx->d_out_cap.release(); ctx->d_out_len.release(); ctx->d_info.release();
     ctx->d_seg_size.release(); ctx->d_payload_len.release(); ctx->d_status.release();
     ctx->d_gtab16.release();
+    ctx->d_walk.release(); ctx->d_desc.release(); ctx->d_bad.release(); ctx->d_content.release();
 #ifdef LZ4B200_AB_VARIANTS
     ctx->d_ttab16.release(); ctx->d_gtag32.release();
 #endif
@@ -808,34 +811,13 @@ const char *lz4b200_ctx_last_kernel(const lz4b200_ctx *ctx, int which)
 
 size_t lz4b200_max_output_size(size_t n) { return 16 + 4 + (size_t)((uint64_t)n * 110 / 100); }
 
-uint32_t lz4b200_xxh32(const uint8_t *data, size_t n, uint32_t seed)
-{
-    Xxh32 h(seed);
-    h.update(data, n);
-    return h.digest();
-}
+uint32_t lz4b200_xxh32(const uint8_t *data, size_t n, uint32_t seed) { return fw::xxh32(data, n, seed); }
 
-void lz4b200_xxh32_reset(lz4b200_xxh32_state *st, uint32_t seed)
-{
-    Xxh32 h(seed);
-    memcpy(st->acc, h.acc, sizeof st->acc);
-    st->fill = 0; st->seed = seed; st->total = 0;
-}
+void lz4b200_xxh32_reset(lz4b200_xxh32_state *st, uint32_t seed) { fw::xxh32_reset(*st, seed); }
 
-void lz4b200_xxh32_update(lz4b200_xxh32_state *st, const uint8_t *data, size_t n)
-{
-    Xxh32 h(st->seed);
-    memcpy(h.acc, st->acc, sizeof st->acc); memcpy(h.buf, st->buf, 16); h.fill = st->fill; h.total = st->total;
-    h.update(data, n);
-    memcpy(st->acc, h.acc, sizeof st->acc); memcpy(st->buf, h.buf, 16); st->fill = h.fill; st->total = h.total;
-}
+void lz4b200_xxh32_update(lz4b200_xxh32_state *st, const uint8_t *data, size_t n) { fw::xxh32_update(*st, data, n); }
 
-uint32_t lz4b200_xxh32_digest(const lz4b200_xxh32_state *st)
-{
-    Xxh32 h(st->seed);
-    memcpy(h.acc, st->acc, sizeof st->acc); memcpy(h.buf, st->buf, 16); h.fill = st->fill; h.total = st->total;
-    return h.digest();
-}
+uint32_t lz4b200_xxh32_digest(const lz4b200_xxh32_state *st) { return fw::xxh32_digest(*st); }
 
 // ---- device batch entry points ----------------------------------------------------------------
 
@@ -1676,62 +1658,325 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
 
 namespace {
 
-struct FrameBlockRef {
-    uint64_t payload_off;     // into the input buffer
-    uint32_t payload_len;
-    uint32_t max_out;         // block size of the owning frame
-    bool stored;
-    uint32_t frame_idx;
-};
-struct FrameRef {
-    uint32_t first_block, nblocks;
-    bool has_size, has_checksum, closed;
-    bool linked = false;      // BlockMode::Linked: blocks may reference the frame's earlier output
-    uint64_t content_size;
-    uint32_t content_checksum;
-};
+constexpr uint32_t kHostWalkChunk = 4096;     // descriptors per frame_walk() call on the host
+constexpr uint32_t kDeviceWalkChunk = 65536;  // descriptors one walk launch records on the device (16 B each)
 
-}  // namespace
+// The frame at in[0, n) in host memory: header and BlockInfo chain.
+void walk_frame_host(const uint8_t *in, size_t n, fw::FrameWalk &w, std::vector<fw::FrameBlockDesc> &blocks)
+{
+    w = fw::FrameWalk{};
+    blocks.clear();
+    while (w.stage != fw::kWalkDone) {
+        const size_t at = blocks.size();
+        blocks.resize(at + kHostWalkChunk);
+        blocks.resize(at + fw::frame_walk(in, n, w, blocks.data() + at, kHostWalkChunk));
+    }
+}
+
+// The block checksum step on the host: the first recorded block whose stored checksum is wrong, or kNoBlock.
+uint32_t first_bad_block_host(const uint8_t *in, const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks)
+{
+    if (!(w.flg & 0x10)) return fw::kNoBlock;
+    for (size_t k = 0; k < blocks.size(); k++)
+        if (!fw::block_checksum_ok(in, blocks[k])) return (uint32_t)k;
+    return fw::kNoBlock;
+}
+
+// The frame at d_in[0, n) in device memory: the walk runs in one GPU thread, kDeviceWalkChunk blocks per launch; only
+// the walk state and the descriptors (16 B per block) come back to the host.  With `verify`, each launch's blocks have
+// their checksums checked on the device and *bad receives the first failing block (kNoBlock: none).
+lz4b200_status walk_frame_device(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, size_t n, bool verify,
+                                 fw::FrameWalk &w, std::vector<fw::FrameBlockDesc> &blocks, uint32_t *bad)
+{
+    w = fw::FrameWalk{};
+    blocks.clear();
+    *bad = fw::kNoBlock;
+    CTX_CUDA(ctx, ctx->d_walk.reserve(1)); CTX_CUDA(ctx, ctx->d_desc.reserve(kDeviceWalkChunk));
+    CTX_CUDA(ctx, ctx->d_bad.reserve(1));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p, &w, sizeof w, cudaMemcpyHostToDevice, s));
+    if (verify) CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bad.p, 0xff, 4, s));
+    while (w.stage != fw::kWalkDone) {
+        const uint64_t first = w.nblocks;
+        frame_walk_kernel<<<1, 1, 0, s>>>(d_in, n, ctx->d_walk.p, ctx->d_desc.p, kDeviceWalkChunk);
+        CTX_CUDA(ctx, cudaGetLastError());
+        if (verify) {
+            block_checksum_kernel<<<kDeviceWalkChunk / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_walk.p, first, ctx->d_bad.p);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+        CTX_CUDA(ctx, cudaMemcpyAsync(&w, ctx->d_walk.p, sizeof w, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        const size_t k = w.nblocks - first;
+        blocks.resize(first + k);
+        if (k) {
+            CTX_CUDA(ctx, cudaMemcpyAsync(blocks.data() + first, ctx->d_desc.p, k * sizeof(fw::FrameBlockDesc),
+                                          cudaMemcpyDeviceToHost, s));
+            CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        }
+    }
+    if (verify && !blocks.empty()) {
+        CTX_CUDA(ctx, cudaMemcpyAsync(bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+    return LZ4B200_OK;
+}
 
 // Upper bound of what one block can decode to: its frame's block size, and never more than 255 output bytes per
 // input byte (a length-extension byte of 0xFF stands for 255 bytes; nothing in the format is denser).
-static inline uint64_t block_decoded_cap(uint64_t payload_len, uint64_t bs)
+inline uint64_t block_decoded_cap(uint64_t payload_len, uint64_t bs)
 {
     return std::min<uint64_t>(bs, payload_len * 255ull + 16ull);
 }
 
-lz4b200_status lz4b200_frame_decoded_bound(const uint8_t *in, size_t n, size_t *bound)
+// Every concatenated frame of in[0, n) (host or, with `device`, device memory), summed over the blocks each walk records.
+// The header's content_size is NOT used: it is untrusted, and a frame whose real size differs must still be delivered
+// in full before ContentLengthError is reported (frame/decompress.rs:312-321).
+lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, size_t n,
+                                        size_t *bound)
 {
-    if (!bound || (!in && n)) return LZ4B200_INVALID_ARGUMENT;
+    fw::FrameWalk w;
+    std::vector<fw::FrameBlockDesc> blocks;
     size_t ip = 0, total = 0;
-    while (ip + 4 <= n) {
-        uint32_t magic = rd32(in + ip);
-        size_t bs; unsigned flg = 0x20;
-        if (magic == 0x184C2102u) { ip += 4; bs = 8u << 20; }
-        else {
-            if (n - ip < 7 || magic != 0x184D2204u) break;
-            flg = in[ip + 4];
-            int id = (in[ip + 5] >> 4) & 7;
-            bs = block_size_bytes(id);
-            if (!bs) break;
-            size_t need = 7 + ((flg & 8) ? 8 : 0) + ((flg & 1) ? 4 : 0);
-            if (n - ip < need) break;
-            ip += need;
+    while (ip < n) {
+        if (device) {
+            uint32_t bad;
+            const lz4b200_status st = walk_frame_device(ctx, s, in + ip, n - ip, false, w, blocks, &bad);
+            if (st != LZ4B200_OK) return st;
+        } else {
+            walk_frame_host(in + ip, n - ip, w, blocks);
         }
-        // The header's content_size is NOT used: it is untrusted, and a frame whose real size differs must still be
-        // delivered in full before ContentLengthError is reported (frame/decompress.rs:312-321).
-        for (;;) {
-            if (n - ip < 4) { ip = n; break; }
-            uint32_t word = rd32(in + ip); ip += 4;
-            if (word == 0) { if (flg & 4) ip += 4; break; }
-            size_t len = word & 0x7fffffffu;
-            total += (word & 0x80000000u) ? len : (size_t)block_decoded_cap(len, bs);
-            ip += len + ((flg & 0x10) ? 4 : 0);
-            if (ip > n) { ip = n; break; }
-        }
+        for (const fw::FrameBlockDesc &b : blocks)
+            total += fw::block_stored(b) ? fw::block_len(b) : (size_t)block_decoded_cap(fw::block_len(b), w.bs);
+        if (w.status != LZ4B200_OK || !w.closed) break;
+        ip += w.ip;
     }
     *bound = total;
     return LZ4B200_OK;
+}
+
+// Decodes the blocks a walk recorded, in groups whose device slots fit the context's frame budget (slots are reused
+// from group to group), so a frame of many short blocks costs O(budget) device memory, not #blocks x block size.
+// `in` and `out` are host memory (each group's payload is staged to the device and its output copied back), or with
+// `device` device memory, read and written in place.  When the frame has a content checksum, `content` (host memory,
+// or device memory with `device`) is carried over each group's output.  *written: the bytes delivered.
+lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, uint8_t *out,
+                                   size_t cap, const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks,
+                                   lz4b200_xxh32_state *content, size_t *written, int *block_status,
+                                   uint64_t *err_expected, uint64_t *err_actual)
+{
+    const uint32_t nb = (uint32_t)blocks.size();
+    const uint64_t bs = w.bs;
+    uint64_t total = 0;
+    *written = 0;
+    if (!nb) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    const bool linked = w.linked && nb > 1;
+    std::vector<uint64_t> h_in_off, h_slot_off, seg, h_soff;
+    std::vector<uint32_t> h_in_len, h_cap, produced, h_first, h_slen;
+    std::vector<uint8_t> h_pick;
+    std::vector<int32_t> status;
+    std::vector<uint64_t> expected;
+    for (uint32_t g0 = 0; g0 < nb;) {
+        // a group: as many blocks as fit the budget (a linked frame is one dependency chain: one group)
+        uint32_t g1 = g0;
+        uint64_t slot_total = 0;
+        while (g1 < nb) {
+            const uint64_t c = fw::block_stored(blocks[g1]) ? 0 : block_decoded_cap(fw::block_len(blocks[g1]), bs);
+            const uint64_t in_span = blocks[g1].payload_off + fw::block_len(blocks[g1]) - blocks[g0].payload_off;
+            if (!linked && g1 > g0 && (slot_total + c > ctx->frame_budget || in_span > ctx->frame_budget)) break;
+            slot_total += (c + 15) & ~15ull;
+            g1++;
+        }
+        const uint32_t gn = g1 - g0;
+        const uint64_t in_lo = blocks[g0].payload_off;
+        const uint64_t in_bytes = blocks[g1 - 1].payload_off + fw::block_len(blocks[g1 - 1]) - in_lo;
+        h_in_off.assign(gn, 0); h_slot_off.assign(gn, 0); h_in_len.assign(gn, 0); h_cap.assign(gn, 0);
+        h_pick.assign(gn, 0); produced.assign(gn, 0); status.assign(gn, 0); expected.assign(gn, 0); seg.assign(gn + 1, 0);
+        uint64_t so = 0;
+        for (uint32_t k = 0; k < gn; k++) {
+            const fw::FrameBlockDesc &b = blocks[g0 + k];
+            const bool stored = fw::block_stored(b);
+            h_in_off[k] = b.payload_off - in_lo;
+            h_in_len[k] = stored ? 0 : fw::block_len(b);                 // stored blocks are only gathered
+            h_pick[k] = stored ? 1 : 0;
+            h_slot_off[k] = so;
+            h_cap[k] = stored ? 0 : (uint32_t)block_decoded_cap(fw::block_len(b), bs);
+            so += ((uint64_t)h_cap[k] + 15) & ~15ull;
+        }
+        const uint8_t *src = in + in_lo;                                   // the group's payload on the device
+        if (!device) {
+            CTX_CUDA(ctx, ctx->d_in.reserve(in_bytes + 16));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in + in_lo, in_bytes, cudaMemcpyHostToDevice, s));
+            src = ctx->d_in.p;
+        }
+        CTX_CUDA(ctx, ctx->d_slots.reserve(so + 16));
+        CTX_CUDA(ctx, ctx->d_in_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_in_len.reserve(gn));
+        CTX_CUDA(ctx, ctx->d_out_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(gn));
+        CTX_CUDA(ctx, ctx->d_out_len.reserve(gn)); CTX_CUDA(ctx, ctx->d_status.reserve(gn));
+        CTX_CUDA(ctx, ctx->d_expected.reserve(gn));
+        CTX_CUDA(ctx, ctx->d_pick.reserve(gn)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(gn + 1));
+        CTX_CUDA(ctx, ctx->d_payload_len.reserve(gn));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, h_in_len.data(), gn * 4, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_off.p, h_slot_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_cap.p, h_cap.data(), gn * 4, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_pick.p, h_pick.data(), gn, cudaMemcpyHostToDevice, s));
+        BatchArgs a{src, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, gn, nullptr};
+        lz4b200_status st;
+        if (linked) {
+            // BlockMode::Linked (frame/decompress.rs:196-222): the blocks of a frame form a dependency chain; the
+            // linked kernel resolves offsets that reach before a block in the outputs of its predecessors
+            h_first.assign(gn, 0); h_slen.assign(gn, 0); h_soff.assign(gn, 0);
+            for (uint32_t k = 0; k < gn; k++) {
+                h_slen[k] = fw::block_stored(blocks[g0 + k]) ? fw::block_len(blocks[g0 + k]) : 0;
+                h_soff[k] = h_in_off[k];
+            }
+            CTX_CUDA(ctx, ctx->d_link_first.reserve(gn)); CTX_CUDA(ctx, ctx->d_stored_len.reserve(gn));
+            CTX_CUDA(ctx, ctx->d_stored_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_done.reserve(gn));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_link_first.p, h_first.data(), gn * 4, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_len.p, h_slen.data(), gn * 4, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_off.p, h_soff.data(), gn * 8, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_done.p, 0, gn * 4, s));
+            a.link_first = ctx->d_link_first.p; a.stored_off = ctx->d_stored_off.p;
+            a.stored_len = ctx->d_stored_len.p; a.done = ctx->d_done.p;
+            a.tickets = ctx->d_tickets;
+            const uint32_t grid = std::min<uint32_t>((gn + 3) / 4, (uint32_t)ctx->sm_count * 8);
+            lz4_decompress_blocks_linked<32><<<grid, 128, 0, s>>>(a);
+            st = ctx->check(cudaGetLastError(), "linked decode launch") ? LZ4B200_OK : LZ4B200_CUDA_ERROR;
+        } else {
+            st = launch_decompress(ctx, a, s);
+        }
+        if (st != LZ4B200_OK) return st;
+        CTX_CUDA(ctx, cudaMemcpyAsync(produced.data(), ctx->d_out_len.p, gn * 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(status.data(), ctx->d_status.p, gn * 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(expected.data(), ctx->d_expected.p, gn * 8, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+
+        // first failing block (stream order) wins over anything the walk found later
+        uint32_t good = gn;
+        for (uint32_t k = 0; k < gn; k++) {
+            if (fw::block_stored(blocks[g0 + k])) { produced[k] = fw::block_len(blocks[g0 + k]); status[k] = 0; continue; }
+            if (status[k] != 0) { good = k; break; }
+        }
+        uint64_t gtotal = 0;
+        for (uint32_t k = 0; k < good; k++) { seg[k] = gtotal; gtotal += produced[k]; }
+        seg[good] = gtotal;
+        if (total + gtotal > cap) { *written = total; return LZ4B200_FRAME_OUTPUT_FULL; }
+        if (gtotal) {
+            uint8_t *dst = out + total;                                    // the device path gathers in place
+            if (!device) {
+                CTX_CUDA(ctx, ctx->d_out.reserve(gtotal + 16));
+                dst = ctx->d_out.p;
+            }
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_seg_off.p, seg.data(), (good + 1) * 8, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_payload_len.p, produced.data(), good * 4, cudaMemcpyHostToDevice, s));
+            GatherArgs g{ctx->d_slots.p, src, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p,
+                         ctx->d_payload_len.p, ctx->d_pick.p, nullptr, dst, ctx->d_seg_off.p, good};
+            gather_segments_kernel<<<std::min<uint32_t>(good, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+            CTX_CUDA(ctx, cudaGetLastError());
+            if (device) {
+                if (w.has_checksum) {
+                    content_hash_kernel<<<1, 256, 0, s>>>(content, out + total, gtotal);
+                    CTX_CUDA(ctx, cudaGetLastError());
+                }
+            } else {
+                CTX_CUDA(ctx, cudaMemcpyAsync(out + total, ctx->d_out.p, gtotal, cudaMemcpyDeviceToHost, s));
+                CTX_CUDA(ctx, cudaStreamSynchronize(s));
+                if (w.has_checksum) fw::xxh32_update(*content, out + total, gtotal);
+            }
+        }
+        total += gtotal;
+        *written = total;
+        if (good < gn) {
+            if (block_status) *block_status = status[good];
+            if (status[good] == LZ4B200_DEC_OUTPUT_TOO_SMALL) {
+                if (err_expected) *err_expected = expected[good];
+                if (err_actual) *err_actual = h_cap[good];
+            }
+            return LZ4B200_FRAME_DECOMPRESSION_ERROR;
+        }
+        g0 = g1;
+    }
+    return LZ4B200_OK;
+}
+
+// One frame, FrameDecoder::read_to_end (frame/decompress.rs:109-342): walk, block checksums, decode, then content size
+// and checksum at the EndMark.  `in` and `out` are host memory, or device memory with `device`; both paths run the same
+// walk and the same group loop, so they return the same result for the same bytes.
+lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, size_t n,
+                                          uint8_t *out, size_t cap, size_t *consumed, size_t *written, int *block_status,
+                                          uint64_t *err_expected, uint64_t *err_actual)
+{
+    *written = 0; *consumed = 0;
+    if (block_status) *block_status = 0;
+    if (err_expected) *err_expected = 0;
+    if (err_actual) *err_actual = 0;
+    if (n == 0) return LZ4B200_OK;                          // read_frame_info: 0 bytes where a frame would start = end of data
+
+    fw::FrameWalk w;
+    std::vector<fw::FrameBlockDesc> blocks;
+    uint32_t bad = fw::kNoBlock;
+    if (device) {
+        const lz4b200_status st = walk_frame_device(ctx, s, in, n, true, w, blocks, &bad);
+        if (st != LZ4B200_OK) return st;
+    } else {
+        walk_frame_host(in, n, w, blocks);
+        bad = first_bad_block_host(in, w, blocks);
+    }
+    if (bad != fw::kNoBlock) {                               // the frame ends at the first block that fails its checksum
+        fw::frame_walk_fail_block(w, blocks[bad], bad);
+        blocks.resize(bad);
+    }
+    *consumed = w.ip;
+
+    lz4b200_xxh32_state content;
+    fw::xxh32_reset(content, 0);
+    lz4b200_xxh32_state *cs = &content;
+    if (device && w.has_checksum && !blocks.empty()) {
+        CTX_CUDA(ctx, ctx->d_content.reserve(1));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_content.p, &content, sizeof content, cudaMemcpyHostToDevice, s));
+        cs = ctx->d_content.p;
+    }
+    size_t total = 0;
+    const lz4b200_status st = decode_frame_blocks(ctx, s, device, in, out, cap, w, blocks, cs, &total, block_status,
+                                                  err_expected, err_actual);
+    *written = total;
+    if (st != LZ4B200_OK) return st;
+    if (w.status != LZ4B200_OK) return (lz4b200_status)w.status;
+
+    // ---- content size / checksum at the EndMark (decompress.rs:312-331) ---------------------------------------------------
+    if (w.closed) {
+        if (w.has_size && total != w.content_size) {
+            if (err_expected) *err_expected = w.content_size;
+            if (err_actual) *err_actual = total;
+            return LZ4B200_FRAME_CONTENT_LENGTH;
+        }
+        if (w.has_checksum) {
+            if (cs != &content) {
+                CTX_CUDA(ctx, cudaMemcpyAsync(&content, cs, sizeof content, cudaMemcpyDeviceToHost, s));
+                CTX_CUDA(ctx, cudaStreamSynchronize(s));
+            }
+            if (fw::xxh32_digest(content) != w.content_checksum) return LZ4B200_FRAME_CONTENT_CHECKSUM;
+        }
+    }
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+lz4b200_status lz4b200_frame_decoded_bound(const uint8_t *in, size_t n, size_t *bound)
+{
+    if (!bound || (!in && n)) return LZ4B200_INVALID_ARGUMENT;
+    return frame_decoded_bound_impl(nullptr, nullptr, false, in, n, bound);
+}
+
+lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
+                                                  void *stream)
+{
+    if (!ctx || !bound || (!d_in && n)) return LZ4B200_INVALID_ARGUMENT;
+    *bound = 0;
+    DeviceGuard guard(ctx->device);
+    return frame_decoded_bound_impl(ctx, (cudaStream_t)stream, true, d_in, n, bound);
 }
 
 void lz4b200_ctx_set_frame_budget(lz4b200_ctx *ctx, size_t bytes)
@@ -1739,210 +1984,30 @@ void lz4b200_ctx_set_frame_budget(lz4b200_ctx *ctx, size_t bytes)
     if (ctx) ctx->frame_budget = std::max<size_t>(bytes, 1u << 20);
 }
 
-// One frame.  Host walk of its header and BlockInfo chain (frame/decompress.rs:109-342), then the blocks are decoded
-// in groups whose device slots fit the context's frame budget (slots are reused from group to group), so a frame of
-// many short blocks costs O(budget) device memory, not #blocks x block size.
+// One frame from host memory into host memory: the walk and the block / content checksums on the CPU, each group's
+// payload staged to the device, decoded, and copied back.
 lz4b200_status lz4b200_frame_decompress_next(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
                                              size_t *consumed, size_t *written, int *block_status,
                                              uint64_t *err_expected, uint64_t *err_actual)
 {
     if (!ctx || !written || !consumed || (!in && n) || (!out && cap)) return LZ4B200_INVALID_ARGUMENT;
-    *written = 0; *consumed = 0;
-    if (block_status) *block_status = 0;
-    if (err_expected) *err_expected = 0;
-    if (err_actual) *err_actual = 0;
-    if (n == 0) return LZ4B200_OK;                          // read_frame_info: 0 bytes where a frame would start = end of data
+    return frame_decompress_next_impl(ctx, ctx->stream, false, in, n, out, cap, consumed, written, block_status,
+                                      err_expected, err_actual);
+}
 
-    // ---- header -----------------------------------------------------------------------------------
-    std::vector<FrameBlockRef> blocks;
-    lz4b200_status walk_err = LZ4B200_OK;
-    size_t ip = 0;
-    size_t bs; unsigned flg = 0x20;
-    FrameRef fr{0, 0, false, false, false, 0, 0};
-    if (n < 4) { *consumed = n; return LZ4B200_FRAME_IO_EOF; }
-    const uint32_t magic = rd32(in);
-    if (magic == 0x184C2102u) {                             // legacy frame: header.rs:285-291
-        ip = 4; bs = 8u << 20;
-    } else {
-        if (n == 4) { *consumed = 4; return LZ4B200_OK; }   // decompress.rs:124-128: nothing after the magic = end of data
-        if (n < 7) { *consumed = n; return LZ4B200_FRAME_IO_EOF; }
-        if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) return LZ4B200_FRAME_SKIPPABLE;
-        if (magic != 0x184D2204u) return LZ4B200_FRAME_WRONG_MAGIC;
-        flg = in[4];
-        const uint8_t bd = in[5];
-        const size_t need = 7 + ((flg & 0x08) ? 8 : 0) + ((flg & 0x01) ? 4 : 0);
-        if (n < need) { *consumed = n; return LZ4B200_FRAME_IO_EOF; }
-        if ((flg & 0xC0) != 0x40) return LZ4B200_FRAME_UNSUPPORTED_VERSION;
-        if ((flg & 0x02) || (bd & 0x8F)) return LZ4B200_FRAME_RESERVED_BITS;
-        const int id = (bd >> 4) & 7;
-        if (id < 4) return LZ4B200_FRAME_UNSUPPORTED_BLOCKSIZE;
-        bs = block_size_bytes(id);
-        size_t o = 6;
-        if (flg & 0x08) { memcpy(&fr.content_size, in + o, 8); fr.has_size = true; o += 8; }
-        if (flg & 0x01) o += 4;
-        if ((uint8_t)(lz4b200_xxh32(in + 4, o - 4, 0) >> 8) != in[o]) return LZ4B200_FRAME_HEADER_CHECKSUM;
-        if (flg & 0x01) return LZ4B200_FRAME_DICTIONARY;
-        fr.linked = !(flg & 0x20);
-        ip = o + 1;
-    }
-    // ---- BlockInfo chain --------------------------------------------------------------------------
-    for (;;) {
-        if (n - ip < 4) { ip = n; break; }                  // EOF where a BlockInfo is due: decompress.rs:236-243
-        const uint32_t word = rd32(in + ip); ip += 4;
-        if (word == 0) {                                     // EndMark
-            fr.closed = true;
-            if (flg & 0x04) {
-                if (n - ip < 4) { walk_err = LZ4B200_FRAME_IO_EOF; ip = n; break; }
-                fr.has_checksum = true; fr.content_checksum = rd32(in + ip); ip += 4;
-            }
-            break;
-        }
-        const size_t len = word & 0x7fffffffu;
-        if (len > bs) { walk_err = LZ4B200_FRAME_BLOCK_TOO_BIG; break; }
-        if (n - ip < len) { walk_err = LZ4B200_FRAME_IO_EOF; ip = n; break; }
-        const size_t payload = ip; ip += len;
-        if (flg & 0x10) {
-            if (n - ip < 4) { walk_err = LZ4B200_FRAME_IO_EOF; ip = n; break; }
-            if (rd32(in + ip) != lz4b200_xxh32(in + payload, len, 0)) { walk_err = LZ4B200_FRAME_BLOCK_CHECKSUM; break; }
-            ip += 4;
-        }
-        blocks.push_back({payload, (uint32_t)len, (uint32_t)bs, (word & 0x80000000u) != 0, 0});
-        fr.nblocks++;
-    }
-    *consumed = ip;
-
-    // ---- decode every block seen before the walk stopped, group by group ---------------------------
-    const uint32_t nb = (uint32_t)blocks.size();
-    uint64_t total = 0;
-    Xxh32 content(0);
-    if (nb) {
-        DeviceGuard guard(ctx->device);
-        cudaStream_t s = ctx->stream;
-        const bool linked = fr.linked && nb > 1;
-        std::vector<uint64_t> h_in_off, h_slot_off, seg, h_soff;
-        std::vector<uint32_t> h_in_len, h_cap, produced, h_first, h_slen;
-        std::vector<uint8_t> h_pick;
-        std::vector<int32_t> status;
-        std::vector<uint64_t> expected;
-        for (uint32_t g0 = 0; g0 < nb;) {
-            // a group: as many blocks as fit the budget (a linked frame is one dependency chain: one group)
-            uint32_t g1 = g0;
-            uint64_t slot_total = 0;
-            while (g1 < nb) {
-                const uint64_t c = blocks[g1].stored ? 0 : block_decoded_cap(blocks[g1].payload_len, bs);
-                const uint64_t in_span = blocks[g1].payload_off + blocks[g1].payload_len - blocks[g0].payload_off;
-                if (!linked && g1 > g0 && (slot_total + c > ctx->frame_budget || in_span > ctx->frame_budget)) break;
-                slot_total += (c + 15) & ~15ull;
-                g1++;
-            }
-            const uint32_t gn = g1 - g0;
-            const uint64_t in_lo = blocks[g0].payload_off;
-            const uint64_t in_bytes = blocks[g1 - 1].payload_off + blocks[g1 - 1].payload_len - in_lo;
-            h_in_off.assign(gn, 0); h_slot_off.assign(gn, 0); h_in_len.assign(gn, 0); h_cap.assign(gn, 0);
-            h_pick.assign(gn, 0); produced.assign(gn, 0); status.assign(gn, 0); expected.assign(gn, 0); seg.assign(gn + 1, 0);
-            uint64_t so = 0;
-            for (uint32_t k = 0; k < gn; k++) {
-                const FrameBlockRef &b = blocks[g0 + k];
-                h_in_off[k] = b.payload_off - in_lo;
-                h_in_len[k] = b.stored ? 0 : b.payload_len;            // stored blocks are only gathered
-                h_pick[k] = b.stored ? 1 : 0;
-                h_slot_off[k] = so;
-                h_cap[k] = b.stored ? 0 : (uint32_t)block_decoded_cap(b.payload_len, bs);
-                so += ((uint64_t)h_cap[k] + 15) & ~15ull;
-            }
-            CTX_CUDA(ctx, ctx->d_in.reserve(in_bytes + 16));
-            CTX_CUDA(ctx, ctx->d_slots.reserve(so + 16));
-            CTX_CUDA(ctx, ctx->d_in_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_in_len.reserve(gn));
-            CTX_CUDA(ctx, ctx->d_out_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(gn));
-            CTX_CUDA(ctx, ctx->d_out_len.reserve(gn)); CTX_CUDA(ctx, ctx->d_status.reserve(gn));
-            CTX_CUDA(ctx, ctx->d_expected.reserve(gn));
-            CTX_CUDA(ctx, ctx->d_pick.reserve(gn)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(gn + 1));
-            CTX_CUDA(ctx, ctx->d_payload_len.reserve(gn));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in + in_lo, in_bytes, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, h_in_len.data(), gn * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_off.p, h_slot_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_cap.p, h_cap.data(), gn * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_pick.p, h_pick.data(), gn, cudaMemcpyHostToDevice, s));
-            BatchArgs a{ctx->d_in.p, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
-                        ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, gn, nullptr};
-            lz4b200_status st;
-            if (linked) {
-                // BlockMode::Linked (frame/decompress.rs:196-222): the blocks of a frame form a dependency chain; the
-                // linked kernel resolves offsets that reach before a block in the outputs of its predecessors
-                h_first.assign(gn, 0); h_slen.assign(gn, 0); h_soff.assign(gn, 0);
-                for (uint32_t k = 0; k < gn; k++) {
-                    h_slen[k] = blocks[g0 + k].stored ? blocks[g0 + k].payload_len : 0;
-                    h_soff[k] = h_in_off[k];
-                }
-                CTX_CUDA(ctx, ctx->d_link_first.reserve(gn)); CTX_CUDA(ctx, ctx->d_stored_len.reserve(gn));
-                CTX_CUDA(ctx, ctx->d_stored_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_done.reserve(gn));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_link_first.p, h_first.data(), gn * 4, cudaMemcpyHostToDevice, s));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_len.p, h_slen.data(), gn * 4, cudaMemcpyHostToDevice, s));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_off.p, h_soff.data(), gn * 8, cudaMemcpyHostToDevice, s));
-                CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_done.p, 0, gn * 4, s));
-                a.link_first = ctx->d_link_first.p; a.stored_off = ctx->d_stored_off.p;
-                a.stored_len = ctx->d_stored_len.p; a.done = ctx->d_done.p;
-                a.tickets = ctx->d_tickets;
-                const uint32_t grid = std::min<uint32_t>((gn + 3) / 4, (uint32_t)ctx->sm_count * 8);
-                lz4_decompress_blocks_linked<32><<<grid, 128, 0, s>>>(a);
-                st = ctx->check(cudaGetLastError(), "linked decode launch") ? LZ4B200_OK : LZ4B200_CUDA_ERROR;
-            } else {
-                st = launch_decompress(ctx, a, s);
-            }
-            if (st != LZ4B200_OK) return st;
-            CTX_CUDA(ctx, cudaMemcpyAsync(produced.data(), ctx->d_out_len.p, gn * 4, cudaMemcpyDeviceToHost, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(status.data(), ctx->d_status.p, gn * 4, cudaMemcpyDeviceToHost, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(expected.data(), ctx->d_expected.p, gn * 8, cudaMemcpyDeviceToHost, s));
-            CTX_CUDA(ctx, cudaStreamSynchronize(s));
-
-            // first failing block (stream order) wins over anything the walk found later
-            uint32_t good = gn;
-            for (uint32_t k = 0; k < gn; k++) {
-                if (blocks[g0 + k].stored) { produced[k] = blocks[g0 + k].payload_len; status[k] = 0; continue; }
-                if (status[k] != 0) { good = k; break; }
-            }
-            uint64_t gtotal = 0;
-            for (uint32_t k = 0; k < good; k++) { seg[k] = gtotal; gtotal += produced[k]; }
-            seg[good] = gtotal;
-            if (total + gtotal > cap) { *written = total; return LZ4B200_FRAME_OUTPUT_FULL; }
-            if (gtotal) {
-                CTX_CUDA(ctx, ctx->d_out.reserve(gtotal + 16));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_seg_off.p, seg.data(), (good + 1) * 8, cudaMemcpyHostToDevice, s));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_payload_len.p, produced.data(), good * 4, cudaMemcpyHostToDevice, s));
-                GatherArgs g{ctx->d_slots.p, ctx->d_in.p, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p,
-                             ctx->d_payload_len.p, ctx->d_pick.p, nullptr, ctx->d_out.p, ctx->d_seg_off.p, good};
-                gather_segments_kernel<<<std::min<uint32_t>(good, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
-                CTX_CUDA(ctx, cudaGetLastError());
-                CTX_CUDA(ctx, cudaMemcpyAsync(out + total, ctx->d_out.p, gtotal, cudaMemcpyDeviceToHost, s));
-                CTX_CUDA(ctx, cudaStreamSynchronize(s));
-                if (fr.has_checksum) content.update(out + total, gtotal);
-            }
-            total += gtotal;
-            *written = total;
-            if (good < gn) {
-                if (block_status) *block_status = status[good];
-                if (status[good] == LZ4B200_DEC_OUTPUT_TOO_SMALL) {
-                    if (err_expected) *err_expected = expected[good];
-                    if (err_actual) *err_actual = h_cap[good];
-                }
-                return LZ4B200_FRAME_DECOMPRESSION_ERROR;
-            }
-            g0 = g1;
-        }
-    }
-    if (walk_err != LZ4B200_OK) return walk_err;
-
-    // ---- content size / checksum at the EndMark (decompress.rs:312-331) -----------------------------
-    if (fr.closed) {
-        if (fr.has_size && total != fr.content_size) {
-            if (err_expected) *err_expected = fr.content_size;
-            if (err_actual) *err_actual = total;
-            return LZ4B200_FRAME_CONTENT_LENGTH;
-        }
-        if (fr.has_checksum && content.digest() != fr.content_checksum) return LZ4B200_FRAME_CONTENT_CHECKSUM;
-    }
-    return LZ4B200_OK;
+// One frame from device memory into device memory: walk, block checksums, decode and content checksum on the GPU; only
+// block descriptors, per-group statuses and the 48-byte hash state cross PCIe.
+lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint8_t *d_out,
+                                                    size_t cap, size_t *consumed, size_t *written, int *block_status,
+                                                    uint64_t *err_expected, uint64_t *err_actual, void *stream)
+{
+    if (!ctx || !written || !consumed || (!d_in && n) || (!d_out && cap)) return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const lz4b200_status st = frame_decompress_next_impl(ctx, s, true, d_in, n, d_out, cap, consumed, written,
+                                                         block_status, err_expected, err_actual);
+    if (st != LZ4B200_CUDA_ERROR) CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    return st;
 }
 
 // Every concatenated frame of `in`, back to back (a convenience over lz4b200_frame_decompress_next: the reference's

@@ -159,6 +159,68 @@ def decompress_frame(data, ctx: _block.Context | None = None, partial: bool = Fa
     return joined
 
 
+def _device_u8(t, what: str):
+    if not (t.is_cuda and t.dtype.itemsize == 1 and t.dim() == 1 and t.is_contiguous()):
+        raise TypeError(f"{what} must be a contiguous 1-D torch CUDA uint8 tensor")
+
+
+def decompress_next_frame_device(d_in, d_out, ctx: _block.Context | None = None, stream: int | None = None):
+    """The frame that starts at d_in[0], decoded from device memory into d_out through
+    lz4b200_frame_decompress_next_device: returns (consumed, written, exception or None), the same values
+    decompress_next_frame() gives for the same bytes in host memory.  d_in and d_out are torch CUDA uint8 tensors;
+    the work runs on torch's current stream (or `stream`) and the call returns once d_out holds the result.  Bytes
+    of d_out past `written` are left untouched."""
+    import torch
+    _device_u8(d_in, "d_in")
+    _device_u8(d_out, "d_out")
+    ctx = ctx or _block.default_context()
+    s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+    n, cap = d_in.numel(), d_out.numel()
+    used, w, bs = C.c_size_t(0), C.c_size_t(0), C.c_int(0)
+    e1, e2 = C.c_uint64(0), C.c_uint64(0)
+    st = _native.lib().lz4b200_frame_decompress_next_device(
+        ctx.handle, d_in.data_ptr() if n else None, n, d_out.data_ptr() if cap else None, cap, C.byref(used),
+        C.byref(w), C.byref(bs), C.byref(e1), C.byref(e2), s)
+    err = None if st == 0 else error_from_status(st, bs.value, ctx.last_cuda_error(), e1.value, e2.value)
+    return used.value, w.value, err
+
+
+def decoded_bound_device(d_in, ctx: _block.Context | None = None, stream: int | None = None) -> int:
+    """Upper bound of the decoded size of every concatenated frame in the device tensor d_in."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+    bound = C.c_size_t(0)
+    st = _native.lib().lz4b200_frame_decoded_bound_device(ctx.handle, d_in.data_ptr() if d_in.numel() else None,
+                                                          d_in.numel(), C.byref(bound), s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return bound.value
+
+
+def decompress_frame_device(d_in, out=None, ctx: _block.Context | None = None):
+    """Every concatenated frame of the device tensor d_in, decoded on the GPU into `out` (a torch CUDA uint8 tensor;
+    None: one of lz4b200_frame_decoded_bound_device bytes is allocated).  Returns the view of `out` that holds the
+    decoded bytes.  Raises what decompress_frame() raises for the same bytes."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    if out is None:
+        out = torch.empty(max(decoded_bound_device(d_in, ctx), 1), dtype=torch.uint8, device=d_in.device)
+    _device_u8(out, "out")
+    pos, total = 0, 0
+    while pos < d_in.numel():
+        used, w, err = decompress_next_frame_device(d_in[pos:], out[total:], ctx)
+        total += w
+        if err is not None:
+            raise err
+        if used == 0:
+            break
+        pos += used
+    return out[:total]
+
+
 # -----------------------------------------------------------------------------------------------------
 # FrameEncoder
 # -----------------------------------------------------------------------------------------------------
