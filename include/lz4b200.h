@@ -272,6 +272,16 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
                                       const lz4b200_frame_info *info, size_t first_write_len,
                                       uint8_t *out, size_t cap, size_t *written);
 
+/* FrameEncoder::with_frame_info(info, w); w.write_all(in); finish() — src/frame/compress.rs:128-187,234-404 — for input in
+ * DEVICE memory, written to DEVICE memory.  For every input, info and first_write_len it returns the status
+ * lz4b200_frame_compress returns, and d_out[0, *d_written) holds the bytes that call writes.  Argument errors are
+ * reported before anything is enqueued.  Otherwise the work is enqueued on `stream` and the call returns without
+ * synchronising; *d_written (a device u64) receives the frame length.  d_in and d_out may have any alignment; bytes of
+ * d_out past the frame are not written. */
+lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                             const lz4b200_frame_info *info, size_t first_write_len,
+                                             uint8_t *d_out, size_t cap, uint64_t *d_written, void *stream);
+
 /* Block-range form used for multi-GPU sharding (SURVEY.md §8e): compress frame blocks
  * [first_block, first_block + nblocks) of a stream cut into `block_size`-byte blocks.  `d_in`
  * points at the first byte of block `first_block` (device memory, `in_len` bytes for this

@@ -111,8 +111,9 @@ __global__ void __launch_bounds__(256) gather_segments_kernel(GatherArgs g)
 }
 
 // Frame encoder bookkeeping for a block range: per block, decide compressed-vs-stored
-// (frame/compress.rs:301-306) and produce BlockInfo word + segment size.
-__global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t n,
+// (frame/compress.rs:301-306) and produce BlockInfo word + segment size.  `trailer` (0, or 4 for a
+// block checksum) is reserved after each payload.
+__global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t n, uint32_t trailer,
                                         uint32_t *info_word, uint8_t *pick_raw, uint32_t *seg_size,
                                         uint32_t *payload_len)
 {
@@ -123,7 +124,7 @@ __global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t
     info_word[i] = stored ? (r | 0x80000000u) : c;
     pick_raw[i] = stored ? 1 : 0;
     payload_len[i] = stored ? r : c;
-    seg_size[i] = 4u + (stored ? r : c);
+    seg_size[i] = 4u + (stored ? r : c) + trailer;
 }
 
 // Descriptor generator for a run of equal-sized blocks cut from one contiguous buffer.
@@ -166,23 +167,130 @@ __global__ void __launch_bounds__(128) block_checksum_kernel(const uint8_t *in, 
     if (!fw::block_checksum_ok(in, desc[i])) atomicMin(bad, (uint32_t)(first + i));
 }
 
-// The content checksum is one XXH32 chain over the whole output (frame/decompress.rs:323-331): thread 0 carries it
-// over each group's output as the group lands.  The other threads of the CTA only stage the bytes through shared
-// memory, so that the chain reads them at shared-memory latency rather than waiting on global memory stripe by stripe.
-constexpr uint32_t kHashStage = 16384;
+// The content checksum is one XXH32 chain over the whole content (frame/compress.rs:320, frame/decompress.rs:323-331).
+// content_hash_kernel carries the state *st over p[0, n) exactly like fw::xxh32_update, a pending partial stripe at
+// entry and exit included: the encoder runs it once over its input, the decoder once per group as the group lands.
+// XXH32 is four serial chains, one per 4-byte lane of a 16-byte stripe, each three dependent instructions per word
+// (multiply-add, rotate, multiply).  Lanes 0-3 of warp 0 each run one chain over words read from shared memory while
+// the other warps stage the next chunk into the second buffer.  The pending stripe is completed byte by byte; the rest
+// is staged in 16-byte words from the 16-byte aligned-down address, the partial words at either end byte by byte, so p
+// may have any alignment and nothing outside p[0, n) is read.
+constexpr uint32_t kHashChunk = 16384;                   // input bytes per staged chunk
+constexpr uint32_t kHashChunkWords = kHashChunk / 16;    // 16-byte words (= stripes) per chunk
+
+// Stage the words of chunk c that hold stripe bytes: word w covers a[16w, 16w + 16); bytes outside [lo, hi) are not
+// read.  A chunk starting `lo` bytes past an aligned address spans one word more than it has stripes.
+__device__ __forceinline__ void hash_stage_chunk(uint8_t *dst, const uint8_t *a, uint64_t lo, uint64_t hi, uint64_t c,
+                                                 uint32_t t, uint32_t nt)
+{
+    const uint64_t w0 = c * kHashChunkWords;
+    const uint64_t w1 = min(w0 + kHashChunkWords + 1, (hi + 15) / 16);
+    for (uint64_t w = w0 + t; w < w1; w += nt) {
+        uint8_t *d = dst + 16 * (w - w0);
+        const uint64_t b = 16 * w;
+        if (b >= lo && b + 16 <= hi) {
+            *reinterpret_cast<uint4 *>(d) = *reinterpret_cast<const uint4 *>(a + b);
+        } else {
+            for (uint32_t i = 0; i < 16; i++)
+                if (b + i >= lo && b + i < hi) d[i] = a[b + i];
+        }
+    }
+}
+
+// One lane's chain over `ns` staged stripes whose first byte is at buf[shift]: word = bytes [off, off + 4) of buf,
+// assembled from the two aligned words around it.
+__device__ __forceinline__ uint32_t hash_chunk_lane(const uint8_t *buf, uint32_t shift, uint32_t lane, uint32_t acc,
+                                                    uint32_t ns)
+{
+    const uint32_t *s32 = reinterpret_cast<const uint32_t *>(buf);
+    const uint32_t r = 8 * (shift & 3);
+    uint32_t i = (shift >> 2) + lane;
+#pragma unroll 8
+    for (uint32_t j = 0; j < ns; j++, i += 4) acc = fw::xxh32_round(acc, __funnelshift_r(s32[i], s32[i + 1], r));
+    return acc;
+}
+
 __global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *st, const uint8_t *p, uint64_t n)
 {
-    __shared__ uint8_t stage[kHashStage];
-    lz4b200_xxh32_state h;
-    if (threadIdx.x == 0) h = *st;
-    for (uint64_t o = 0; o < n; o += kHashStage) {
-        const uint32_t len = n - o < kHashStage ? (uint32_t)(n - o) : kHashStage;
-        for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) stage[i] = p[o + i];
-        __syncthreads();
-        if (threadIdx.x == 0) fw::xxh32_update(h, stage, len);
+    __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
+    const uint32_t fill = st->fill;
+    const uint64_t k = fill ? min((uint64_t)(16u - fill), n) : 0;
+    __syncthreads();                                              // every thread has read fill before it changes
+    if (threadIdx.x == 0 && k) fw::xxh32_update(*st, p, k);     // complete (or extend) the pending stripe
+    __syncthreads();
+    const bool pending = st->fill != 0;                           // n too short to complete it: nothing else to do
+    uint32_t acc = st->acc[threadIdx.x & 3];
+    __syncthreads();                                              // every thread has read *st before it is written
+    if (pending) return;
+
+    const uint8_t *q = p + k;
+    const uint64_t m = n - k, stripes = m >> 4;
+    const uint32_t shift = (uint32_t)(reinterpret_cast<uintptr_t>(q) & 15u);
+    const uint8_t *a = q - shift;                                 // 16-byte aligned
+    const uint64_t lo = shift, hi = shift + 16 * stripes;         // the stripes' bytes, relative to a
+    const uint64_t nchunks = (stripes + kHashChunkWords - 1) / kHashChunkWords;
+    if (nchunks) hash_stage_chunk(stage[0], a, lo, hi, 0, threadIdx.x, blockDim.x);
+    __syncthreads();
+    for (uint64_t c = 0; c < nchunks; c++) {
+        if (threadIdx.x < 32) {
+            if (threadIdx.x < 4)
+                acc = hash_chunk_lane(stage[c & 1], shift, threadIdx.x, acc,
+                                      (uint32_t)min((uint64_t)kHashChunkWords, stripes - c * kHashChunkWords));
+        } else if (c + 1 < nchunks) {
+            hash_stage_chunk(stage[(c + 1) & 1], a, lo, hi, c + 1, threadIdx.x - 32, blockDim.x - 32);
+        }
         __syncthreads();
     }
-    if (threadIdx.x == 0) *st = h;
+    if (threadIdx.x < 4) st->acc[threadIdx.x] = acc;
+    if (threadIdx.x == 0) {
+        const uint32_t tail = (uint32_t)(m & 15);
+        for (uint32_t i = 0; i < tail; i++) st->buf[i] = q[16 * stripes + i];
+        st->fill = tail;
+        st->total += m;
+    }
+}
+
+// ---- device-resident frame encoder (lz4b200_frame_compress_device) ------------------------------------------------------
+
+__global__ void xxh32_reset_kernel(lz4b200_xxh32_state *st, uint32_t seed) { fw::xxh32_reset(*st, seed); }
+
+// Block checksums of a packed range (frame/compress.rs:313-316): the XXH32 of each payload as written (compressed or
+// stored), stored little-endian in the 4 trailer bytes after it.  One thread per block.
+__global__ void __launch_bounds__(128) frame_block_checksum_kernel(uint8_t *dst, const uint64_t *seg_off,
+                                                                   const uint32_t *payload_len, uint32_t n)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint8_t *payload = dst + seg_off[i] + 4;
+    const uint32_t len = payload_len[i];
+    const uint32_t h = fw::xxh32(payload, len, 0);
+    for (int b = 0; b < 4; b++) payload[len + b] = (uint8_t)(h >> (8 * b));
+}
+
+// The frame header as a kernel argument (FrameInfo::write is at most 15 bytes).
+struct FrameHeaderBytes {
+    uint8_t b[19];
+    uint8_t len;
+};
+
+// Everything of the frame but its blocks (frame/compress.rs:209-230, header.rs:232-275): the header at out[0], the
+// EndMark after the *seg_total bytes of blocks (null: none), the content digest when `content` is given, and the frame
+// length into *written.
+__global__ void frame_tail_kernel(uint8_t *out, FrameHeaderBytes hdr, const uint64_t *seg_total,
+                                  const lz4b200_xxh32_state *content, uint64_t *written)
+{
+#pragma unroll
+    for (uint32_t i = 0; i < sizeof hdr.b; i++)
+        if (i < hdr.len) out[i] = hdr.b[i];
+    uint64_t o = hdr.len + (seg_total ? *seg_total : 0);
+    for (int b = 0; b < 4; b++) out[o + b] = 0;
+    o += 4;
+    if (content) {
+        const uint32_t h = fw::xxh32_digest(*content);
+        for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
+        o += 4;
+    }
+    *written = o;
 }
 
 }  // namespace lz4b200
@@ -1485,11 +1593,17 @@ size_t lz4b200_frame_bound(size_t n, const lz4b200_frame_info *info)
     return 19 + n + nb * 8 + 8;
 }
 
+}  // extern "C"
+
+namespace {
+
 // Rank-local half of a (possibly sharded) frame, step 1: compress the blocks of [first_block, ...) into the context's
-// slots, decide compressed-vs-stored per block (frame/compress.rs:301-306) and scan the segment sizes.  *d_total
-// receives the packed size.  Everything stays on the device and on `stream`.
-lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
-                                            uint64_t first_block, uint64_t *d_total, uint32_t *d_block_sizes, void *stream)
+// slots, decide compressed-vs-stored per block (frame/compress.rs:301-306) and scan the segment sizes, each of which
+// reserves `trailer` bytes (0, or 4 for a block checksum) after its payload.  *d_total receives the packed size.
+// Everything stays on the device and on `stream`.
+lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
+                                         uint64_t first_block, uint32_t trailer, uint64_t *d_total,
+                                         uint32_t *d_block_sizes, void *stream)
 {
     if (!ctx || !block_size || block_size > (8u << 20)) return LZ4B200_INVALID_ARGUMENT;
     const size_t nblocks = (in_len + block_size - 1) / block_size;
@@ -1520,8 +1634,9 @@ lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_i
                 ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
     lz4b200_status st = launch_compress(ctx, a, (uint32_t)std::min<size_t>(block_size, in_len), s);
     if (st != LZ4B200_OK) return st;
-    frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb, ctx->d_info.p,
-                                                            ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
+    frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb, trailer,
+                                                            ctx->d_info.p, ctx->d_pick.p, ctx->d_seg_size.p,
+                                                            ctx->d_payload_len.p);
     CTX_CUDA(ctx, cudaGetLastError());
     scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);
     CTX_CUDA(ctx, cudaGetLastError());
@@ -1529,6 +1644,16 @@ lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_i
     if (d_block_sizes)
         CTX_CUDA(ctx, cudaMemcpyAsync(d_block_sizes, ctx->d_seg_size.p, nb * 4, cudaMemcpyDeviceToDevice, s));
     return LZ4B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
+                                            uint64_t first_block, uint64_t *d_total, uint32_t *d_block_sizes, void *stream)
+{
+    return frame_range_compress_impl(ctx, d_in, in_len, block_size, first_block, 0, d_total, d_block_sizes, stream);
 }
 
 // Step 2: pack the range's [BlockInfo | payload] segments back to back at d_dst + *d_dst_offset.  d_dst may be PEER
@@ -1653,6 +1778,58 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
     wr32(out + o, 0); o += 4;                                                            // EndMark: compress.rs:221-223
     if (info.content_checksum) { wr32(out + o, lz4b200_xxh32(in, n, 0)); o += 4; }       // compress.rs:224-227
     *written = o;
+    return LZ4B200_OK;
+}
+
+// lz4b200_frame_compress for input in device memory, written to device memory without a host synchronisation: the
+// blocks are compressed and packed at d_out + header length with room for their checksums, which one thread per block
+// then writes; the content hash runs over d_in in the context's d_content state; one tail kernel writes the header
+// (a kernel argument), the EndMark, the content digest and *d_written.  Only kernel arguments cross PCIe.
+lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                             const lz4b200_frame_info *info_in, size_t first_write_len, uint8_t *d_out,
+                                             size_t cap, uint64_t *d_written, void *stream)
+{
+    if (!ctx || !info_in || !d_out || !d_written || (!d_in && n)) return LZ4B200_INVALID_ARGUMENT;
+    lz4b200_frame_info info = *info_in;
+    if (info.linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    if (info.block_size_id == 0) info.block_size_id = auto_block_size_id(first_write_len);   // compress.rs:236-238
+    if (info.block_size_id < 4 || info.block_size_id > 7) return LZ4B200_INVALID_ARGUMENT;
+    if (info.has_content_size && info.content_size != n) return LZ4B200_FRAME_CONTENT_LENGTH; // compress.rs:212-219
+    const size_t bs = block_size_bytes(info.block_size_id);
+    if (cap < lz4b200_frame_bound(n, &info)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+
+    FrameHeaderBytes hdr{};
+    hdr.len = (uint8_t)lz4b200_frame_write_header(&info, hdr.b, sizeof hdr.b);
+    const uint64_t *seg_total = nullptr;
+    if (n) {
+        lz4b200_status st = frame_range_compress_impl(ctx, d_in, n, bs, 0, info.block_checksums ? 4u : 0u, nullptr,
+                                                      nullptr, s);
+        if (st != LZ4B200_OK) return st;
+        st = lz4b200_frame_range_pack(ctx, d_out + hdr.len, nullptr, s);
+        if (st != LZ4B200_OK) return st;
+        const uint32_t nb = ctx->range_nb;
+        if (info.block_checksums) {
+            frame_block_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_out + hdr.len, ctx->d_seg_off.p,
+                                                                         ctx->d_payload_len.p, nb);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+        seg_total = ctx->d_seg_off.p + nb;
+    }
+    const lz4b200_xxh32_state *content = nullptr;
+    if (info.content_checksum) {                                                         // compress.rs:141,320
+        CTX_CUDA(ctx, ctx->d_content.reserve(1));
+        xxh32_reset_kernel<<<1, 1, 0, s>>>(ctx->d_content.p, 0);
+        CTX_CUDA(ctx, cudaGetLastError());
+        if (n) {
+            content_hash_kernel<<<1, 256, 0, s>>>(ctx->d_content.p, d_in, n);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+        content = ctx->d_content.p;
+    }
+    frame_tail_kernel<<<1, 1, 0, s>>>(d_out, hdr, seg_total, content, d_written);
+    CTX_CUDA(ctx, cudaGetLastError());
     return LZ4B200_OK;
 }
 

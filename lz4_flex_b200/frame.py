@@ -6,6 +6,8 @@ FrameInfo / BlockSize / BlockMode / FrameEncoder / FrameDecoder with the referen
 and decompressed in GPU batches through the C ABI.  Block boundaries, the stored-raw rule and — crucially —
 each block's parse mode (FRESH for the first block of a table epoch, CONT afterwards, SURVEY.md §8a) follow
 FrameEncoder::write/write_block exactly, so the produced frame is byte-identical to lz4_flex's.
+For data already in GPU memory, compress_frame_device() and decompress_frame_device() keep the whole container on the
+device: header, EndMark and both checksums are written or verified by kernels, and no payload crosses PCIe.
 
 BlockMode::Linked chains every block to its frame's earlier output.  The DECODER handles it on the device
 (lz4_decompress_blocks_linked: a block waits for the predecessors an offset reaches into), so frames written by
@@ -119,6 +121,38 @@ def compress_frame(data, frame_info: FrameInfo | None = None, ctx: _block.Contex
     if st != 0:
         raise error_from_status(st, detail=ctx.last_cuda_error())
     return out[: w.value].tobytes()
+
+
+def compress_frame_device(d_in, frame_info: FrameInfo | None = None, out=None, ctx: _block.Context | None = None,
+                          stream: int | None = None):
+    """compress_frame() for input in device memory, through lz4b200_frame_compress_device: the frame is written to
+    `out` (a contiguous 1-D torch CUDA uint8 tensor; None: one of lz4b200_frame_bound bytes is allocated) and the view
+    of `out` that holds it is returned, byte-identical to what compress_frame() gives for the same bytes.  The work,
+    checksums included, runs on torch's current stream (or `stream`); the call returns once the frame length has been
+    read back.  Raises what compress_frame() raises for the same arguments."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    info = frame_info or FrameInfo()
+    if info.block_mode == BlockMode.Linked:
+        raise LinkedBlocksUnsupported()
+    ci = info.to_c()
+    n = d_in.numel()
+    if out is None:
+        out = torch.empty(_native.lib().lz4b200_frame_bound(n, C.byref(ci)), dtype=torch.uint8, device=d_in.device)
+    _device_u8(out, "out")
+    s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+    written = torch.empty(1, dtype=torch.int64, device=out.device)
+    st = _native.lib().lz4b200_frame_compress_device(ctx.handle, d_in.data_ptr() if n else None, n, C.byref(ci), n,
+                                                     out.data_ptr(), out.numel(), written.data_ptr(), s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    if stream is None:
+        w = int(written.item())
+    else:
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=out.device)):
+            w = int(written.item())                                           # copied and synchronised on `stream`
+    return out[:w]
 
 
 def decompress_next_frame(data, ctx: _block.Context | None = None):
