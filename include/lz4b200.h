@@ -101,7 +101,10 @@ void lz4b200_ctx_set_priority(lz4b200_ctx *ctx, int high);
 /* The context's own stream (cudaStream_t). */
 void *lz4b200_ctx_stream(lz4b200_ctx *ctx);
 /* Name of the kernel the launcher picked for the context's last compress (which = 0) / decompress (which = 1) batch —
- * diagnostics only: bench.py records it beside the roofline so a profile is never attributed to the wrong kernel. */
+ * diagnostics only: bench.py records it beside the roofline so a profile is never attributed to the wrong kernel.  The name
+ * carries the template arguments of the instantiation that ran.  A compress batch whose `max_in_len` exceeds 64 KiB
+ * names the encoder of blocks above 64 KiB; one with `max_in_len` 0, or whose dictionary takes dict_len + max_in_len
+ * above 64 KiB, runs that encoder as well as the one of the smaller blocks and names both, joined by " + ". */
 const char *lz4b200_ctx_last_kernel(const lz4b200_ctx *ctx, int which);
 
 /* ---- sizes ------------------------------------------------------------------------------ */

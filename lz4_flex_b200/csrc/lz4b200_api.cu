@@ -394,6 +394,7 @@ struct lz4b200_ctx {
 #endif
     std::string last_error;
     const char *last_kernel[2] = {"", ""};   // what the launchers picked last: [0] compress, [1] decompress (for the bench record)
+    std::string last_kernel_both;             // storage of last_kernel[0] when the u16 and u32 encoders both ran
     uint32_t range_nb = 0;                    // lz4b200_frame_range_compress -> _pack hand-over
     const uint8_t *range_in = nullptr;
     size_t frame_budget = 256u << 20;         // device bytes the frame decoder's block slots / staged input may take per group
@@ -485,8 +486,11 @@ lz4b200_status launch_decompress_g(lz4b200_ctx *ctx, const BatchArgs &a, cudaStr
     if (one_warp) lz4_decompress_blocks<G, 0, false, 1><<<warps, 32, 0, s>>>(a);
     else if (a.dict_len) lz4_decompress_blocks<G, 0, true><<<grid, kDecWarpsPerCta * 32, 0, s>>>(a);
     else lz4_decompress_blocks<G, 0, false><<<grid, kDecWarpsPerCta * 32, 0, s>>>(a);
-    ctx->last_kernel[1] = one_warp ? (G == 8 ? "lz4_decompress_blocks<8, 0, 0, 1>" : G == 16 ? "lz4_decompress_blocks<16, 0, 0, 1>" : "lz4_decompress_blocks<32, 0, 0, 1>")
-                                   : (G == 8 ? "lz4_decompress_blocks<8, 0, 0, 4>" : G == 16 ? "lz4_decompress_blocks<16, 0, 0, 4>" : "lz4_decompress_blocks<32, 0, 0, 4>");
+#define LZ4B200_DEC_NAME(g, d, w) "lz4_decompress_blocks<" #g ", 0, " #d ", " w ">"
+    ctx->last_kernel[1] = one_warp ? (G == 8 ? LZ4B200_DEC_NAME(8, 0, "1") : G == 16 ? LZ4B200_DEC_NAME(16, 0, "1") : LZ4B200_DEC_NAME(32, 0, "1"))
+        : a.dict_len ? (G == 8 ? LZ4B200_DEC_NAME(8, 1, LZ4B200_STR(DEC_WARPS_PER_CTA)) : G == 16 ? LZ4B200_DEC_NAME(16, 1, LZ4B200_STR(DEC_WARPS_PER_CTA)) : LZ4B200_DEC_NAME(32, 1, LZ4B200_STR(DEC_WARPS_PER_CTA)))
+                     : (G == 8 ? LZ4B200_DEC_NAME(8, 0, LZ4B200_STR(DEC_WARPS_PER_CTA)) : G == 16 ? LZ4B200_DEC_NAME(16, 0, LZ4B200_STR(DEC_WARPS_PER_CTA)) : LZ4B200_DEC_NAME(32, 0, LZ4B200_STR(DEC_WARPS_PER_CTA)));
+#undef LZ4B200_DEC_NAME
     CTX_CUDA(ctx, cudaGetLastError());
     return LZ4B200_OK;
 }
@@ -692,7 +696,8 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
                 ctx->last_kernel[0] = kGtabKernelName;
             }
         } else {
-            ctx->last_kernel[0] = "lz4_compress_blocks_split<unsigned short, 3, 0>";
+            ctx->last_kernel[0] = a.dict_len ? "lz4_compress_blocks_split<unsigned short, " LZ4B200_STR(ENC16_PAIRS) ", 1>"
+                                             : "lz4_compress_blocks_split<unsigned short, " LZ4B200_STR(ENC16_PAIRS) ", 0>";
             const uint32_t grid = std::min<uint32_t>((a.nblocks + kEnc16Pairs - 1) / kEnc16Pairs, (uint32_t)(ctx->sm_count * ctx->enc16s_ctas_per_sm));
             if (a.dict_len)
                 lz4_compress_blocks_split<uint16_t, kEnc16Pairs, true>
@@ -704,7 +709,16 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
         CTX_CUDA(ctx, cudaGetLastError());
     }
     if (max_in_len == 0 || (uint64_t)max_in_len + a.dict_len > 65536u) {
-        if (max_in_len > 65536u) ctx->last_kernel[0] = "lz4_compress_blocks_split<unsigned int, 2, 0>";
+        // a bound above 64 KiB names the large-block kernel alone; an unknown bound, or a dictionary that takes the span
+        // above 64 KiB, leaves work for both kernels, and the record names both in launch order
+        static_assert(kEnc32Pairs == 2, "the kernel names below spell out kEnc32Pairs");
+        const char *k32 = a.dict_len ? "lz4_compress_blocks_split<unsigned int, 2, 1>" : "lz4_compress_blocks_split<unsigned int, 2, 0>";
+        if (max_in_len > 65536u) {
+            ctx->last_kernel[0] = k32;
+        } else {
+            ctx->last_kernel_both = std::string(ctx->last_kernel[0]) + " + " + k32;
+            ctx->last_kernel[0] = ctx->last_kernel_both.c_str();
+        }
         const uint32_t grid = std::min<uint32_t>((a.nblocks + kEnc32Pairs - 1) / kEnc32Pairs, (uint32_t)(ctx->sm_count * ctx->enc32s_ctas_per_sm));
         if (a.dict_len)
             lz4_compress_blocks_split<uint32_t, kEnc32Pairs, true>
