@@ -366,6 +366,32 @@ lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint
 lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
                                                   void *stream);
 
+/* What lz4b200_frame_decompress_next returns for one frame: its status and its five result scalars. */
+typedef struct lz4b200_frame_result {
+    uint64_t consumed, written, err_expected, err_actual;
+    int32_t status, block_status;
+} lz4b200_frame_result;                          /* 40 bytes */
+
+/* Many independent frames in DEVICE memory, decoded into DEVICE memory in one call.  Frame f is the frame that starts
+ * at d_in + d_frame_off[f], in a region of d_frame_len[f] bytes; d_results[f] receives exactly what
+ * lz4b200_frame_decompress_next returns on the same context (same frame budget) for those bytes in host memory with
+ * cap = d_out_cap[f], and d_out[d_out_off[f], +written) the bytes it writes.  Nothing else of d_out is written.  A
+ * region that holds several concatenated frames decodes only the first (`consumed` says where it ended).  Output
+ * regions must not overlap (not checked).  Every array is in device memory.  INVALID_ARGUMENT, before anything is
+ * enqueued: a null ctx, a null array with nframes > 0, nframes > UINT32_MAX; nframes == 0 does nothing.  A frame's own
+ * error goes into its result and does not affect any other frame.  The frames' blocks are decoded together, many
+ * frames per launch; the call synchronises `stream` before it returns. */
+lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+    uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+    lz4b200_frame_result *d_results, size_t nframes, void *stream);
+
+/* d_bound[f] = what lz4b200_frame_decoded_bound gives for region f when it holds one frame (the first frame's bound
+ * when it holds several).  Enqueued on `stream`; the call returns without synchronising.  Argument errors as above. */
+lz4b200_status lz4b200_frame_decoded_bound_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+    uint64_t *d_bound, size_t nframes, void *stream);
+
 /* XXH32 (twox-hash XxHash32, Cargo.toml:51) — used for header/block/content checksums.
  * The streaming form backs FrameEncoder's running content hash (frame/compress.rs:141,320). */
 uint32_t lz4b200_xxh32(const uint8_t *data, size_t n, uint32_t seed);

@@ -149,6 +149,8 @@ SIGNATURES = {
     "lz4b200_frame_decompress_next_device": (_i32, [_vp, _vp, _sz, _vp, _sz, _psz, _psz, C.POINTER(C.c_int),
                                                     C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), _vp]),
     "lz4b200_frame_decoded_bound_device": (_i32, [_vp, _vp, _sz, _psz, _vp]),
+    "lz4b200_frame_decompress_batch_device": (_i32, [_vp] * 8 + [_sz, _vp]),
+    "lz4b200_frame_decoded_bound_batch_device": (_i32, [_vp] * 5 + [_sz, _vp]),
     "lz4b200_ctx_set_frame_budget": (None, [_vp, _sz]),
     "lz4b200_xxh32": (_u32, [_vp, _sz, _u32]),
     "lz4b200_xxh32_reset": (None, [_vp, _u32]),

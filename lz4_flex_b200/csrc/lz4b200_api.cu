@@ -210,9 +210,11 @@ __device__ __forceinline__ uint32_t hash_chunk_lane(const uint8_t *buf, uint32_t
     return acc;
 }
 
-__global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *st, const uint8_t *p, uint64_t n)
+// The body of content_hash_kernel, run by every thread of a CTA (shared by the per-frame hash of the batch decoder):
+// carries *st (global or shared memory) over p[0, n) using the two staging buffers.
+__device__ __forceinline__ void content_hash_cta(lz4b200_xxh32_state *st, const uint8_t *p, uint64_t n,
+                                                 uint8_t (*stage)[kHashChunk + 16])
 {
-    __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
     const uint32_t fill = st->fill;
     const uint64_t k = fill ? min((uint64_t)(16u - fill), n) : 0;
     __syncthreads();                                              // every thread has read fill before it changes
@@ -248,6 +250,12 @@ __global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *
         st->fill = tail;
         st->total += m;
     }
+}
+
+__global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *st, const uint8_t *p, uint64_t n)
+{
+    __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
+    content_hash_cta(st, p, n, stage);
 }
 
 // ---- device-resident frame encoder (lz4b200_frame_compress_device) ------------------------------------------------------
@@ -291,6 +299,194 @@ __global__ void frame_tail_kernel(uint8_t *out, FrameHeaderBytes hdr, const uint
         o += 4;
     }
     *written = o;
+}
+
+// ---- batch frame decoder (lz4b200_frame_decompress_batch_device) --------------------------------------------------------
+// Many independent frames per call.  Frame f is the one that starts at in + frame_off[f] in a region of frame_len[f]
+// bytes.  The host plans groups of whole frames from a count walk; per group, blocks are indexed frame after frame, the
+// blocks of independent frames first and those of linked frames after them (descriptor index `base` of a frame).
+
+// Count walk, one thread per frame: the walk state, the count, and the block count per class (independent blocks at
+// nb2[f], linked at nb2[n + f]) for the descriptor scans.
+__global__ void __launch_bounds__(128) frame_count_kernel(const uint8_t *in, const uint64_t *frame_off,
+                                                          const uint64_t *frame_len, uint32_t n, uint64_t budget,
+                                                          fw::FrameWalk *walks, fw::FrameCount *counts, uint32_t *nb2)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    fw::FrameWalk w;
+    fw::FrameCount c;
+    fw::frame_count(in + frame_off[f], frame_len[f], w, c, budget);
+    walks[f] = w;
+    counts[f] = c;
+    const uint32_t nb = (uint32_t)c.nblocks;                      // the host sends larger frames down the one-frame path
+    nb2[f] = c.linked ? 0u : nb;
+    nb2[n + f] = c.linked ? nb : 0u;
+}
+
+// lz4b200_frame_decoded_bound of the first frame of each region, one thread per region.
+__global__ void __launch_bounds__(128) frame_bound_kernel(const uint8_t *in, const uint64_t *frame_off,
+                                                          const uint64_t *frame_len, uint32_t n, uint64_t *bound)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    fw::FrameWalk w;
+    fw::FrameBlockDesc buf[4];
+    uint64_t total = 0;
+    while (w.stage != fw::kWalkDone) {
+        const uint32_t k = fw::frame_walk(in + frame_off[f], frame_len[f], w, buf, 4);
+        for (uint32_t i = 0; i < k; i++)
+            total += fw::block_stored(buf[i]) ? fw::block_len(buf[i]) : fw::block_decoded_cap(fw::block_len(buf[i]), w.bs);
+    }
+    bound[f] = total;
+}
+
+// Record walk of the group's frames [f0, f0 + gn), one thread per frame: each frame's descriptors at its base (from the
+// scans of the two block-count classes), and per block its frame and slot bytes.
+__global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, const uint64_t *frame_off,
+                                                           const uint64_t *frame_len, uint32_t f0, uint32_t gn,
+                                                           const fw::FrameWalk *walks, const fw::FrameCount *counts,
+                                                           const uint64_t *scan_ind, const uint64_t *scan_lnk,
+                                                           fw::FrameBlockDesc *desc, uint32_t *fbase, uint32_t *bframe,
+                                                           uint32_t *bslot, uint32_t *bad)
+{
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= gn) return;
+    const uint32_t f = f0 + g;
+    const fw::FrameCount c = counts[f];
+    const uint32_t base = (uint32_t)(c.linked ? scan_ind[gn] + scan_lnk[g] : scan_ind[g]);
+    fw::FrameWalk w;
+    const uint32_t nb = fw::frame_walk(in + frame_off[f], frame_len[f], w, desc + base, (uint32_t)c.nblocks);
+    for (uint32_t k = 0; k < nb; k++) {
+        bframe[base + k] = g;
+        bslot[base + k] = (uint32_t)fw::slot_bytes(fw::block_slot_cap(desc[base + k], walks[f].bs));
+    }
+    fbase[g] = base;
+    bad[g] = fw::kNoBlock;
+}
+
+// Block checksums, one thread per block of the group; bad[g] receives the first failing block of frame g.
+__global__ void __launch_bounds__(128) frame_batch_checksum_kernel(const uint8_t *in, const uint64_t *frame_off,
+                                                                   uint32_t f0, const fw::FrameWalk *walks,
+                                                                   const fw::FrameBlockDesc *desc, const uint32_t *fbase,
+                                                                   const uint32_t *bframe, uint32_t nb, uint32_t *bad)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    const uint32_t g = bframe[b];
+    if (!(walks[f0 + g].flg & 0x10)) return;
+    if (!fw::block_checksum_ok(in + frame_off[f0 + g], desc[b])) atomicMin(bad + g, b - fbase[g]);
+}
+
+// The decoder's arguments, one thread per block of the group: blocks at and past a frame's first bad block are not
+// decoded (in_len 0, cap 0, like a stored block) and nothing of theirs is delivered.  Linked blocks (index >= nind)
+// also get their chain start relative to the linked launch's first block.
+__global__ void __launch_bounds__(128) frame_batch_args_kernel(const uint64_t *frame_off, uint32_t f0,
+                                                               const fw::FrameWalk *walks, const fw::FrameBlockDesc *desc,
+                                                               const uint32_t *fbase, const uint32_t *bframe,
+                                                               const uint32_t *bad, uint32_t nb, uint32_t nind,
+                                                               uint64_t *in_off, uint32_t *in_len, uint32_t *out_cap,
+                                                               uint8_t *pick, uint32_t *link_first, uint32_t *stored_len,
+                                                               uint32_t *done)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    const uint32_t g = bframe[b];
+    const fw::FrameBlockDesc d = desc[b];
+    const bool live = b - fbase[g] < bad[g], stored = fw::block_stored(d), decode = live && !stored;
+    in_off[b] = frame_off[f0 + g] + d.payload_off;
+    in_len[b] = decode ? fw::block_len(d) : 0u;
+    out_cap[b] = decode ? (uint32_t)fw::block_decoded_cap(fw::block_len(d), walks[f0 + g].bs) : 0u;
+    pick[b] = decode ? 0 : 1;
+    if (b >= nind) {
+        link_first[b] = fbase[g] - nind;
+        stored_len[b] = live && stored ? fw::block_len(d) : 0u;
+        done[b] = 0;
+    }
+}
+
+// One thread per frame of the group: the group loop's result for a frame that is one group (decode_frame_blocks, then
+// frame_decompress_next_impl's checks at the EndMark), and the gather of its delivered blocks.  hash[g] is set, and
+// states[g] reset, when the result still depends on the content checksum.
+__global__ void __launch_bounds__(128) frame_resolve_kernel(uint32_t f0, uint32_t gn, const fw::FrameWalk *walks,
+                                                            const fw::FrameCount *counts, const fw::FrameBlockDesc *desc,
+                                                            const uint32_t *fbase, const uint32_t *bad,
+                                                            const uint32_t *out_len, const int32_t *status,
+                                                            const uint64_t *expected, const uint32_t *blk_cap,
+                                                            const uint64_t *frame_out_off, const uint64_t *frame_out_cap,
+                                                            uint64_t *dst_off, uint32_t *glen, uint8_t *hash,
+                                                            lz4b200_xxh32_state *states, lz4b200_frame_result *results)
+{
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= gn) return;
+    const uint32_t f = f0 + g, base = fbase[g], nrec = (uint32_t)counts[f].nblocks;
+    fw::FrameWalk w = walks[f];
+    if (bad[g] != fw::kNoBlock) fw::frame_walk_fail_block(w, desc[base + bad[g]], bad[g]);
+    const uint32_t nb = (uint32_t)w.nblocks;
+    lz4b200_frame_result r{};
+    r.consumed = w.ip;
+    uint32_t good = nb;
+    uint64_t total = 0;
+    for (uint32_t k = 0; k < nrec; k++) {                   // the first failing block in stream order ends the output
+        const uint32_t b = base + k;
+        uint32_t len = 0;
+        if (k < good) {
+            if (fw::block_stored(desc[b])) len = fw::block_len(desc[b]);
+            else if (status[b] != 0) good = k;
+            else len = out_len[b];
+        }
+        dst_off[b] = frame_out_off[f] + total;
+        glen[b] = len;
+        total += len;
+    }
+    uint8_t h = 0;
+    if (total > frame_out_cap[f]) {                         // checked before the decode error, as the group loop does
+        r.status = LZ4B200_FRAME_OUTPUT_FULL;
+        for (uint32_t k = 0; k < nrec; k++) glen[base + k] = 0;
+    } else {
+        r.written = total;
+        if (good < nb) {
+            const uint32_t b = base + good;
+            r.status = LZ4B200_FRAME_DECOMPRESSION_ERROR;
+            r.block_status = status[b];
+            if (status[b] == LZ4B200_DEC_OUTPUT_TOO_SMALL) { r.err_expected = expected[b]; r.err_actual = blk_cap[b]; }
+        } else if (w.status != LZ4B200_OK) {
+            r.status = w.status;
+        } else if (w.closed) {
+            if (w.has_size && total != w.content_size) {
+                r.status = LZ4B200_FRAME_CONTENT_LENGTH;
+                r.err_expected = w.content_size;
+                r.err_actual = total;
+            } else if (w.has_checksum) {
+                h = 1;
+                fw::xxh32_reset(states[g], 0);
+            }
+        }
+    }
+    hash[g] = h;
+    results[f] = r;
+}
+
+// The content hash of each frame of the group that still needs one, one CTA per frame over its delivered output, carried
+// in states[g] (reset by the resolve step); frame_batch_digest_kernel then compares the digests.
+// frame_out_off and results start at the group's first frame.  (The minimum of one CTA per SM lifts the 40-register
+// limit ptxas otherwise picks here, which spills; it runs at 55 registers, four CTAs per SM.)
+__global__ void __launch_bounds__(256, 1) frame_batch_hash_kernel(const uint8_t *out, const uint64_t *frame_out_off,
+                                                               const uint8_t *hash, lz4b200_xxh32_state *states,
+                                                               const lz4b200_frame_result *results)
+{
+    __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
+    const uint32_t g = blockIdx.x;
+    if (hash[g]) content_hash_cta(states + g, out + frame_out_off[g], results[g].written, stage);
+}
+
+__global__ void __launch_bounds__(128) frame_batch_digest_kernel(uint32_t f0, uint32_t gn, const fw::FrameWalk *walks,
+                                                                 const uint8_t *hash, const lz4b200_xxh32_state *states,
+                                                                 lz4b200_frame_result *results)
+{
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < gn && hash[g] && fw::xxh32_digest(states[g]) != walks[f0 + g].content_checksum)
+        results[f0 + g].status = LZ4B200_FRAME_CONTENT_CHECKSUM;
 }
 
 }  // namespace lz4b200
@@ -411,6 +607,13 @@ struct lz4b200_ctx {
     DevBuf<fw::FrameBlockDesc> d_desc;
     DevBuf<uint32_t> d_bad;
     DevBuf<lz4b200_xxh32_state> d_content;
+    // batch frame decoder: per frame the walk, the count and the two block counts; per group the scans, the frames'
+    // descriptor bases, first bad blocks and hash flags; per block its frame, slot bytes and gather lengths
+    DevBuf<fw::FrameWalk> d_fwalk;
+    DevBuf<fw::FrameCount> d_fcount;
+    DevBuf<uint32_t> d_fnb, d_fbase, d_fbad, d_bframe, d_bslot, d_glen;
+    DevBuf<uint64_t> d_fscan, d_gdst;
+    DevBuf<uint8_t> d_fhash;
 
     bool check(cudaError_t e, const char *what)
     {
@@ -1911,13 +2114,6 @@ lz4b200_status walk_frame_device(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t
     return LZ4B200_OK;
 }
 
-// Upper bound of what one block can decode to: its frame's block size, and never more than 255 output bytes per
-// input byte (a length-extension byte of 0xFF stands for 255 bytes; nothing in the format is denser).
-inline uint64_t block_decoded_cap(uint64_t payload_len, uint64_t bs)
-{
-    return std::min<uint64_t>(bs, payload_len * 255ull + 16ull);
-}
-
 // Every concatenated frame of in[0, n) (host or, with `device`, device memory), summed over the blocks each walk records.
 // The header's content_size is NOT used: it is untrusted, and a frame whose real size differs must still be delivered
 // in full before ContentLengthError is reported (frame/decompress.rs:312-321).
@@ -1936,7 +2132,7 @@ lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool d
             walk_frame_host(in + ip, n - ip, w, blocks);
         }
         for (const fw::FrameBlockDesc &b : blocks)
-            total += fw::block_stored(b) ? fw::block_len(b) : (size_t)block_decoded_cap(fw::block_len(b), w.bs);
+            total += fw::block_stored(b) ? fw::block_len(b) : (size_t)fw::block_decoded_cap(fw::block_len(b), w.bs);
         if (w.status != LZ4B200_OK || !w.closed) break;
         ip += w.ip;
     }
@@ -1971,10 +2167,10 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
         uint32_t g1 = g0;
         uint64_t slot_total = 0;
         while (g1 < nb) {
-            const uint64_t c = fw::block_stored(blocks[g1]) ? 0 : block_decoded_cap(fw::block_len(blocks[g1]), bs);
+            const uint64_t c = fw::block_slot_cap(blocks[g1], bs);
             const uint64_t in_span = blocks[g1].payload_off + fw::block_len(blocks[g1]) - blocks[g0].payload_off;
-            if (!linked && g1 > g0 && (slot_total + c > ctx->frame_budget || in_span > ctx->frame_budget)) break;
-            slot_total += (c + 15) & ~15ull;
+            if (!linked && g1 > g0 && fw::group_cut(slot_total, c, in_span, ctx->frame_budget)) break;
+            slot_total += fw::slot_bytes(c);
             g1++;
         }
         const uint32_t gn = g1 - g0;
@@ -1990,8 +2186,8 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
             h_in_len[k] = stored ? 0 : fw::block_len(b);                 // stored blocks are only gathered
             h_pick[k] = stored ? 1 : 0;
             h_slot_off[k] = so;
-            h_cap[k] = stored ? 0 : (uint32_t)block_decoded_cap(fw::block_len(b), bs);
-            so += ((uint64_t)h_cap[k] + 15) & ~15ull;
+            h_cap[k] = (uint32_t)fw::block_slot_cap(b, bs);
+            so += fw::slot_bytes(h_cap[k]);
         }
         const uint8_t *src = in + in_lo;                                   // the group's payload on the device
         if (!device) {
@@ -2153,6 +2349,76 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
     return LZ4B200_OK;
 }
 
+// A group of the batch: frames [f0, f0 + gn), each of which the group loop decodes as one group, with nind blocks of
+// independent frames and nlnk of linked frames whose slots take `slots` bytes.  Record walk, block checksums, one
+// decode launch per class, resolve, one gather and the per-frame content hash, all enqueued on s.
+lz4b200_status decode_frame_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off,
+                                  const uint64_t *d_frame_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                  const uint64_t *d_out_cap, lz4b200_frame_result *d_results, uint32_t nframes,
+                                  uint32_t f0, uint32_t gn, uint32_t nind, uint32_t nlnk, uint64_t slots)
+{
+    const uint32_t nb = nind + nlnk;
+    const uint32_t fgrid = (gn + 127) / 128, bgrid = (nb + 127) / 128;
+    CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_fbase.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_fbad.reserve(gn)); CTX_CUDA(ctx, ctx->d_fhash.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_content.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb)); CTX_CUDA(ctx, ctx->d_bslot.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb + 1)); CTX_CUDA(ctx, ctx->d_slots.reserve(slots + 16));
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_pick.reserve(nb)); CTX_CUDA(ctx, ctx->d_link_first.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_stored_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_done.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    uint64_t *scan_ind = ctx->d_fscan.p, *scan_lnk = ctx->d_fscan.p + gn + 1;
+
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + f0, scan_ind, gn);
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + nframes + f0, scan_lnk, gn);
+    frame_record_kernel<<<fgrid, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, f0, gn, ctx->d_fwalk.p, ctx->d_fcount.p,
+                                              scan_ind, scan_lnk, ctx->d_desc.p, ctx->d_fbase.p, ctx->d_bframe.p,
+                                              ctx->d_bslot.p, ctx->d_fbad.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        frame_batch_checksum_kernel<<<bgrid, 128, 0, s>>>(d_in, d_frame_off, f0, ctx->d_fwalk.p, ctx->d_desc.p,
+                                                          ctx->d_fbase.p, ctx->d_bframe.p, nb, ctx->d_fbad.p);
+        scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_bslot.p, ctx->d_out_off.p, nb);
+        frame_batch_args_kernel<<<bgrid, 128, 0, s>>>(d_frame_off, f0, ctx->d_fwalk.p, ctx->d_desc.p, ctx->d_fbase.p,
+                                                      ctx->d_bframe.p, ctx->d_fbad.p, nb, nind, ctx->d_in_off.p,
+                                                      ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_pick.p,
+                                                      ctx->d_link_first.p, ctx->d_stored_len.p, ctx->d_done.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, nind, nullptr};
+        const lz4b200_status st = launch_decompress(ctx, a, s);
+        if (st != LZ4B200_OK) return st;
+        if (nlnk) {
+            // every linked chain of the group in one launch: block b waits only for blocks [link_first[b], b) of its frame
+            BatchArgs l{d_in, ctx->d_in_off.p + nind, ctx->d_in_len.p + nind, nullptr, ctx->d_slots.p,
+                        ctx->d_out_off.p + nind, ctx->d_out_cap.p + nind, ctx->d_out_len.p + nind,
+                        ctx->d_status.p + nind, ctx->d_expected.p + nind, nlnk, ctx->d_tickets};
+            l.link_first = ctx->d_link_first.p + nind; l.stored_off = ctx->d_in_off.p + nind;
+            l.stored_len = ctx->d_stored_len.p + nind; l.done = ctx->d_done.p + nind;
+            lz4_decompress_blocks_linked<32><<<std::min<uint32_t>((nlnk + 3) / 4, (uint32_t)ctx->sm_count * 8), 128, 0, s>>>(l);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    frame_resolve_kernel<<<fgrid, 128, 0, s>>>(f0, gn, ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_desc.p, ctx->d_fbase.p,
+                                               ctx->d_fbad.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p,
+                                               ctx->d_out_cap.p, d_out_off, d_out_cap, ctx->d_gdst.p, ctx->d_glen.p,
+                                               ctx->d_fhash.p, ctx->d_content.p, d_results);
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_glen.p, ctx->d_glen.p,
+                     ctx->d_pick.p, nullptr, d_out, ctx->d_gdst.p, nb};
+        gather_segments_kernel<<<std::min<uint32_t>(nb, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    frame_batch_hash_kernel<<<gn, 256, 0, s>>>(d_out, d_out_off + f0, ctx->d_fhash.p, ctx->d_content.p, d_results + f0);
+    frame_batch_digest_kernel<<<fgrid, 128, 0, s>>>(f0, gn, ctx->d_fwalk.p, ctx->d_fhash.p, ctx->d_content.p, d_results);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
 }  // namespace
 
 lz4b200_status lz4b200_frame_decoded_bound(const uint8_t *in, size_t n, size_t *bound)
@@ -2199,6 +2465,100 @@ lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint
                                                          block_status, err_expected, err_actual);
     if (st != LZ4B200_CUDA_ERROR) CTX_CUDA(ctx, cudaStreamSynchronize(s));
     return st;
+}
+
+// Many frames from device memory into device memory.  One thread per frame counts its blocks; the host cuts the batch
+// into groups of whole frames whose slots fit the frame budget, each decoded as the one-frame group loop would decode
+// the frame, but with every frame's blocks in the same launches.  A frame that the group loop would split into several
+// groups (at least one budget of slots) goes through the one-frame device call instead.
+lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_frame_off,
+                                                     const uint64_t *d_frame_len, uint8_t *d_out,
+                                                     const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                     lz4b200_frame_result *d_results, size_t nframes, void *stream)
+{
+    if (!ctx || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_frame_off || !d_frame_len || !d_out || !d_out_off || !d_out_cap || !d_results))
+        return LZ4B200_INVALID_ARGUMENT;
+    if (!nframes) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t n = (uint32_t)nframes;
+    CTX_CUDA(ctx, ctx->d_fwalk.reserve(n)); CTX_CUDA(ctx, ctx->d_fcount.reserve(n));
+    CTX_CUDA(ctx, ctx->d_fnb.reserve(2 * (size_t)n));
+    frame_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ctx->frame_budget,
+                                                       ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_fnb.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    std::vector<fw::FrameCount> counts(n);
+    CTX_CUDA(ctx, cudaMemcpyAsync(counts.data(), ctx->d_fcount.p, n * sizeof(fw::FrameCount), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+
+    // groups of consecutive one-group frames whose slots fit the budget (a linked frame larger than the budget is a group
+    // of its own, as in the group loop); at most kGroupItems frames plus blocks per group bound the descriptor arrays
+    constexpr uint64_t kGroupItems = 1u << 20;
+    std::vector<uint32_t> solo;
+    uint32_t g0 = 0, nind = 0, nlnk = 0;                   // the open group is frames [g0, f)
+    uint64_t slots = 0, items = 0;
+    auto flush = [&](uint32_t f) {
+        const lz4b200_status st = f > g0 ? decode_frame_group(ctx, s, d_in, d_frame_off, d_frame_len, d_out, d_out_off,
+                                                              d_out_cap, d_results, n, g0, f - g0, nind, nlnk, slots)
+                                         : LZ4B200_OK;
+        g0 = f; nind = nlnk = 0; slots = items = 0;
+        return st;
+    };
+    for (uint32_t f = 0; f < n; f++) {
+        const fw::FrameCount &c = counts[f];
+        const bool batch = c.one_group && c.nblocks < kGroupItems;
+        if (!batch || slots + c.slot_total > ctx->frame_budget || items + 1 + c.nblocks > kGroupItems) {
+            const lz4b200_status st = flush(f);
+            if (st != LZ4B200_OK) return st;
+        }
+        if (!batch) { solo.push_back(f); g0 = f + 1; continue; }
+        (c.linked ? nlnk : nind) += (uint32_t)c.nblocks;
+        slots += c.slot_total;
+        items += 1 + c.nblocks;
+    }
+    const lz4b200_status st = flush(n);
+    if (st != LZ4B200_OK) return st;
+    if (!solo.empty()) {
+        // frames the group loop splits (at least one budget of slots) or with more blocks than a group holds: the
+        // one-frame device call, which runs the group loop over them
+        std::vector<uint64_t> off(n), len(n), ooff(n), ocap(n);
+        CTX_CUDA(ctx, cudaMemcpyAsync(off.data(), d_frame_off, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(len.data(), d_frame_len, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ooff.data(), d_out_off, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ocap.data(), d_out_cap, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        std::vector<lz4b200_frame_result> res(solo.size());
+        for (size_t i = 0; i < solo.size(); i++) {
+            const uint32_t f = solo[i];
+            lz4b200_frame_result &r = res[i];
+            size_t consumed = 0, written = 0;
+            int bs = 0;
+            r.status = frame_decompress_next_impl(ctx, s, true, d_in + off[f], len[f], d_out + ooff[f], ocap[f],
+                                                  &consumed, &written, &bs, &r.err_expected, &r.err_actual);
+            if (r.status == LZ4B200_CUDA_ERROR) return LZ4B200_CUDA_ERROR;
+            r.consumed = consumed; r.written = written; r.block_status = bs;
+            CTX_CUDA(ctx, cudaMemcpyAsync(d_results + f, &r, sizeof r, cudaMemcpyHostToDevice, s));
+        }
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    return LZ4B200_OK;
+}
+
+// lz4b200_frame_decoded_bound of the first frame of every region, on the GPU; enqueued on `stream`.
+lz4b200_status lz4b200_frame_decoded_bound_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                        const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+                                                        uint64_t *d_bound, size_t nframes, void *stream)
+{
+    if (!ctx || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_frame_off || !d_frame_len || !d_bound)) return LZ4B200_INVALID_ARGUMENT;
+    if (!nframes) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    const uint32_t n = (uint32_t)nframes;
+    frame_bound_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_in, d_frame_off, d_frame_len, n, d_bound);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
 }
 
 // Every concatenated frame of `in`, back to back (a convenience over lz4b200_frame_decompress_next: the reference's

@@ -205,5 +205,58 @@ FW_FN void frame_walk_fail_block(FrameWalk &w, const FrameBlockDesc &b, uint32_t
     w.has_checksum = 0;
 }
 
+// ---- group planning, shared by the one-frame group loop and the batch decoder -------------------------------------------
+// Upper bound of what one block can decode to: its frame's block size, and never more than 255 output bytes per
+// input byte (a length-extension byte of 0xFF stands for 255 bytes; nothing in the format is denser).
+FW_FN uint64_t block_decoded_cap(uint64_t payload_len, uint64_t bs)
+{
+    const uint64_t c = payload_len * 255ull + 16ull;
+    return bs < c ? bs : c;
+}
+// The device slot a block decodes into: its cap rounded up to 16 bytes (stored blocks are only gathered: none).
+FW_FN uint64_t block_slot_cap(const FrameBlockDesc &b, uint64_t bs) { return block_stored(b) ? 0 : block_decoded_cap(block_len(b), bs); }
+FW_FN uint64_t slot_bytes(uint64_t cap) { return (cap + 15) & ~15ull; }
+
+// The group loop's cut: a group that already holds blocks whose slots take `slot_total` bytes ends before a block
+// whose slot needs `cap` bytes, or whose payload ends `in_span` bytes past the group's first payload, when either would
+// pass the budget.
+FW_FN bool group_cut(uint64_t slot_total, uint64_t cap, uint64_t in_span, uint64_t budget)
+{
+    return slot_total + cap > budget || in_span > budget;
+}
+
+// What the batch decoder plans with for one frame (32 bytes): its blocks, their slot bytes, whether it is decoded as
+// one linked chain, and whether the group loop would decode it as one group (linked frames always are).
+struct FrameCount {
+    uint64_t slot_total = 0;
+    uint64_t nblocks = 0;
+    uint64_t first_off = 0;        // payload offset of block 0
+    uint8_t linked = 0, one_group = 1;
+};
+
+// Adds the next block (stream order) of a frame to its count.
+FW_FN void frame_count_add(FrameCount &c, const FrameBlockDesc &b, uint64_t bs, uint64_t budget)
+{
+    const uint64_t cap = block_slot_cap(b, bs);
+    if (c.nblocks == 0) c.first_off = b.payload_off;
+    else if (group_cut(c.slot_total, cap, b.payload_off + block_len(b) - c.first_off, budget)) c.one_group = 0;
+    c.slot_total += slot_bytes(cap);
+    c.nblocks++;
+}
+
+// The whole walk of the frame at in[0, n) with a small descriptor buffer, keeping only the count; w is left as the walk
+// ends (before any block checksum is checked).
+FW_FN void frame_count(const uint8_t *in, uint64_t n, FrameWalk &w, FrameCount &c, uint64_t budget)
+{
+    FrameBlockDesc buf[4];
+    c = FrameCount{};
+    while (w.stage != kWalkDone) {
+        const uint32_t k = frame_walk(in, n, w, buf, 4);
+        for (uint32_t i = 0; i < k; i++) frame_count_add(c, buf[i], w.bs, budget);
+    }
+    if (w.linked) c.one_group = 1;                  // one dependency chain: the group loop never cuts it
+    c.linked = w.linked && c.nblocks > 1;
+}
+
 }  // namespace fw
 }  // namespace lz4b200

@@ -255,6 +255,93 @@ def decompress_frame_device(d_in, out=None, ctx: _block.Context | None = None):
     return out[:total]
 
 
+def _device_i64(v, device, what: str):
+    import torch
+    t = v if isinstance(v, torch.Tensor) else torch.as_tensor(np.asarray(v, dtype=np.int64))
+    t = t.to(device=device, dtype=torch.int64).contiguous()
+    if t.dim() != 1:
+        raise TypeError(f"{what} must be 1-D")
+    return t
+
+
+@dataclass
+class DecodedFrames:
+    """What decompress_frames_device() returns: the output buffer, each frame's output offset, and one row per frame
+    of lz4b200_frame_result as int64 (consumed, written, err_expected, err_actual, status | block_status << 32)."""
+    out: "object"
+    out_offsets: "object"
+    results: "object"
+    _host: Optional[np.ndarray] = None
+
+    def __len__(self) -> int:
+        return self.results.shape[0]
+
+    def frame(self, i: int):
+        """(view of frame i's decoded bytes in `out`, consumed, exception or None): the values
+        decompress_next_frame_device() gives for the same frame."""
+        if self._host is None:
+            self._host = self.results.cpu().numpy()
+            self._offs = self.out_offsets.cpu().numpy()
+        consumed, written, e1, e2, packed = (int(x) for x in self._host[i])
+        st = int(np.int32(packed & 0xFFFFFFFF))
+        bs = int(np.int32((packed >> 32) & 0xFFFFFFFF))
+        err = None if st == 0 else error_from_status(st, bs, "", e1, e2)
+        o = int(self._offs[i])
+        return self.out[o:o + written], consumed, err
+
+    def __iter__(self):
+        return (self.frame(i) for i in range(len(self)))
+
+
+def decompress_frames_device(d_in, offsets, lengths, out=None, out_offsets=None, out_caps=None,
+                             ctx: _block.Context | None = None, stream: int | None = None) -> DecodedFrames:
+    """Many independent frames in the device tensor d_in, decoded on the GPU in one call
+    (lz4b200_frame_decompress_batch_device): frame i is the one that starts at d_in[offsets[i]] in a region of
+    lengths[i] bytes, and is decoded into out[out_offsets[i]:] with room for out_caps[i] bytes.  With out=None each
+    region gets lz4b200_frame_decoded_bound_batch_device bytes, laid out back to back.  d_in and out are contiguous
+    1-D torch CUDA uint8 tensors; offsets, lengths and caps are int64 tensors or sequences.  The work runs on torch's
+    current stream (or `stream`); the call returns once `out` holds the result.  Frame i's result is exactly what
+    decompress_next_frame_device() returns for it: see DecodedFrames.frame()."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    offs, lens = _device_i64(offsets, dev, "offsets"), _device_i64(lengths, dev, "lengths")
+    n = offs.numel()
+    if lens.numel() != n:
+        raise ValueError("offsets and lengths differ in length")
+    if (out is None) != (out_offsets is None) or (out is None) != (out_caps is None):
+        raise ValueError("out, out_offsets and out_caps go together")
+    if out is not None:
+        _device_u8(out, "out")
+        oo, caps = _device_i64(out_offsets, dev, "out_offsets"), _device_i64(out_caps, dev, "out_caps")
+        if oo.numel() != n or caps.numel() != n:
+            raise ValueError("out_offsets and out_caps need one entry per frame")
+    else:
+        caps = torch.zeros(n, dtype=torch.int64, device=dev)
+    results = torch.zeros((n, 5), dtype=torch.int64, device=dev)
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    L = _native.lib()
+    in_ptr = d_in.data_ptr() if d_in.numel() else None
+    if out is None:
+        st = L.lz4b200_frame_decoded_bound_batch_device(ctx.handle, in_ptr, offs.data_ptr(), lens.data_ptr(),
+                                                        caps.data_ptr(), n, s)
+        if st != 0:
+            raise error_from_status(st, detail=ctx.last_cuda_error())
+        with torch.cuda.stream(torch.cuda.ExternalStream(s, device=dev)):
+            ends = torch.cumsum(caps, 0)
+            oo = ends - caps
+            total = int(ends[-1].item()) if n else 0
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    st = L.lz4b200_frame_decompress_batch_device(ctx.handle, in_ptr, offs.data_ptr(), lens.data_ptr(), out.data_ptr(),
+                                                 oo.data_ptr(), caps.data_ptr(), results.data_ptr(), n, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return DecodedFrames(out, oo, results)
+
+
 # -----------------------------------------------------------------------------------------------------
 # FrameEncoder
 # -----------------------------------------------------------------------------------------------------
