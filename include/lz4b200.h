@@ -285,6 +285,29 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
                                              const lz4b200_frame_info *info, size_t first_write_len,
                                              uint8_t *d_out, size_t cap, uint64_t *d_written, void *stream);
 
+/* FrameEncoder::with_frame_info(info_f, w); w.write_all(in_f); finish() for each of many inputs in DEVICE memory, written
+ * back to back into DEVICE memory in one call.  Input f is d_in[in_off[f], in_off[f] + in_len[f]); in_off and in_len are
+ * HOST arrays of nframes entries, d_frame_off a DEVICE array of nframes + 1.  info_f is *info with two changes: block
+ * size Auto (0) resolves from in_len[f] (an Auto batch mixes block sizes), and with has_content_size set frame f's
+ * header records in_len[f] (info->content_size is ignored).  d_out[d_frame_off[f], d_frame_off[f + 1]) holds exactly
+ * the bytes lz4b200_frame_compress(ctx, host copy of input f, in_len[f], &info_f, in_len[f], ...) writes; frames lie
+ * back to back from d_out[0], d_frame_off[nframes] is the total, and nothing of d_out past it is written.
+ * Argument errors, reported before anything is enqueued (d_out and d_frame_off untouched), in this order:
+ *   INVALID_ARGUMENT           a null ctx, info or d_frame_off; a null in_off, in_len or d_out with nframes > 0; a null
+ *                              d_in with a non-empty input;
+ *   FRAME_LINKED_UNSUPPORTED   linked blocks;
+ *   INVALID_ARGUMENT           a block size id other than 0 or 4..7; nframes or the batch's block count above UINT32_MAX;
+ *   COMPRESS_OUTPUT_TOO_SMALL  out_cap < the sum of lz4b200_frame_bound(in_len[f], &info_f).
+ * nframes == 0 sets d_frame_off[0] = 0.  Otherwise all planning is done on the host, the work is enqueued on `stream`
+ * and the call returns without synchronising; calls on one context must be ordered on one stream, as for every device
+ * call.  d_in and d_out may have any alignment and must not overlap.  Device scratch is one slot of
+ * lz4b200_max_output_size(block length) per block, about the size of the input; there is no budget. */
+lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *in_off, const uint64_t *in_len,
+    const lz4b200_frame_info *info,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
+    size_t nframes, void *stream);
+
 /* Block-range form used for multi-GPU sharding (SURVEY.md §8e): compress frame blocks
  * [first_block, first_block + nblocks) of a stream cut into `block_size`-byte blocks.  `d_in`
  * points at the first byte of block `first_block` (device memory, `in_len` bytes for this

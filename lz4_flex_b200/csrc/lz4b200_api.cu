@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "lz4b200_frame_batch.cuh"
 #include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
 #include "lz4b200_solo_kernel.cuh"
@@ -299,6 +300,69 @@ __global__ void frame_tail_kernel(uint8_t *out, FrameHeaderBytes hdr, const uint
         o += 4;
     }
     *written = o;
+}
+
+// ---- batch frame encoder (lz4b200_frame_compress_batch_device) ----------------------------------------------------------
+// Many frames per call, their blocks numbered frame after frame (fb::FramePlan, one entry per frame, planned on the host).
+
+static_assert(sizeof(fb::FramePlan) == 64, "one frame's plan is 64 bytes");
+
+// The compressor's arguments, one thread per block of the batch (fb::batch_block); dst[b] receives the block's shift
+// into the packed output, to which frame_batch_dst_kernel adds the scan of the segment sizes.
+__global__ void __launch_bounds__(128) frame_batch_blocks_kernel(const fb::FramePlan *plan, uint32_t nframes, uint32_t nb,
+                                                                 uint64_t *in_off, uint32_t *in_len, uint64_t *out_off,
+                                                                 uint32_t *out_cap, uint8_t *flags, uint64_t *dst)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    const fb::BlockJob j = fb::batch_block(plan, nframes, b);
+    in_off[b] = j.in_off;
+    in_len[b] = j.in_len;
+    out_off[b] = j.out_off;
+    out_cap[b] = j.out_cap;
+    flags[b] = j.flags;
+    dst[b] = j.dst_shift;
+}
+
+__global__ void __launch_bounds__(128) frame_batch_dst_kernel(const uint64_t *seg_off, uint32_t nb, uint64_t *dst)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < nb) dst[b] += seg_off[b];
+}
+
+// The content hash of every frame (frame/compress.rs:141,320), one CTA per frame over its input, into states[f].
+// (As for frame_batch_hash_kernel, the minimum of one CTA per SM keeps ptxas from a register limit that spills.)
+__global__ void __launch_bounds__(256, 1) frame_batch_content_kernel(const uint8_t *in, const fb::FramePlan *plan,
+                                                                  lz4b200_xxh32_state *states)
+{
+    __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
+    const uint32_t f = blockIdx.x;
+    if (threadIdx.x == 0) fw::xxh32_reset(states[f], 0);
+    __syncthreads();
+    content_hash_cta(states + f, in + plan[f].in_off, plan[f].in_len, stage);
+}
+
+// Everything of each frame but its blocks, one thread per frame (frame/compress.rs:209-230): the header, the EndMark,
+// the content digest when `states` is given, and frame_off[f]; the last frame's thread also writes the total.
+__global__ void __launch_bounds__(128) frame_batch_tail_kernel(uint8_t *out, const fb::FramePlan *plan, uint32_t n,
+                                                               const uint64_t *seg_off, const lz4b200_xxh32_state *states,
+                                                               uint64_t *frame_off)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    const fb::FramePlan &p = plan[f];
+    uint64_t start, o;
+    fb::frame_place(p, seg_off, &start, &o);
+    for (uint32_t i = 0; i < p.hdr_len; i++) out[start + i] = p.hdr[i];
+    for (int b = 0; b < 4; b++) out[o + b] = 0;
+    o += 4;
+    if (states) {
+        const uint32_t h = fw::xxh32_digest(states[f]);
+        for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
+        o += 4;
+    }
+    frame_off[f] = start;
+    if (f == n - 1) frame_off[n] = o;
 }
 
 // ---- batch frame decoder (lz4b200_frame_decompress_batch_device) --------------------------------------------------------
@@ -614,6 +678,7 @@ struct lz4b200_ctx {
     DevBuf<uint32_t> d_fnb, d_fbase, d_fbad, d_bframe, d_bslot, d_glen;
     DevBuf<uint64_t> d_fscan, d_gdst;
     DevBuf<uint8_t> d_fhash;
+    DevBuf<fb::FramePlan> d_fplan;            // batch frame encoder: the host's plan, one entry per frame
 
     bool check(cudaError_t e, const char *what)
     {
@@ -2046,6 +2111,112 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
         content = ctx->d_content.p;
     }
     frame_tail_kernel<<<1, 1, 0, s>>>(d_out, hdr, seg_total, content, d_written);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+// lz4b200_frame_compress_device for each of many inputs, frames packed back to back, in one call.  The host plans every
+// frame (fb::plan_frame) and uploads the plan with one copy from pageable memory, which cudaMemcpyAsync stages before it
+// returns, so back-to-back calls never share a host buffer.  Then, all on `stream`: one thread per block writes the
+// compressor's arguments, one launch compresses every block of every frame, the segment sizes are scanned, one gather
+// packs every [BlockInfo | payload] at its frame's place, one thread per block writes the block checksums, one CTA per
+// frame hashes its content, and one thread per frame writes its header, EndMark, digest and offset.
+lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *in_off,
+                                                   const uint64_t *in_len, const lz4b200_frame_info *info,
+                                                   uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
+                                                   size_t nframes, void *stream)
+{
+    if (!ctx || !info || !d_frame_off || (nframes && (!in_off || !in_len || !d_out))) return LZ4B200_INVALID_ARGUMENT;
+    if (!d_in)
+        for (size_t f = 0; f < nframes; f++)
+            if (in_len[f]) return LZ4B200_INVALID_ARGUMENT;
+    if (info->linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    const int id = info->block_size_id;
+    if ((id != 0 && (id < 4 || id > 7)) || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    const uint32_t tail = info->content_checksum ? 8u : 4u;
+    std::vector<fb::FramePlan> plan(nframes);
+    uint64_t nblocks = 0, bound = 0, slots = 0, max_len = 0;
+    bool small = false;                                     // some block has at most 64 KiB
+    for (size_t f = 0; f < nframes; f++) {
+        lz4b200_frame_info fi = *info;
+        if (id == 0) fi.block_size_id = auto_block_size_id(in_len[f]);                      // compress.rs:236-238
+        fi.content_size = in_len[f];
+        fb::FramePlan &p = plan[f];
+        p.in_off = in_off[f];
+        p.in_len = in_len[f];
+        p.bs = (uint32_t)block_size_bytes(fi.block_size_id);
+        p.fresh = (uint32_t)fresh_period(p.bs);
+        p.hdr_len = (uint8_t)lz4b200_frame_write_header(&fi, p.hdr, sizeof p.hdr);
+        const uint64_t nb = fb::frame_blocks(p);
+        if (nblocks + nb > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+        fb::plan_frame(p, f ? &plan[f - 1] : nullptr, tail);
+        nblocks += nb;
+        bound += lz4b200_frame_bound(p.in_len, &fi);
+        slots += fb::frame_slot_bytes(p);
+        if (nb) {
+            max_len = std::max<uint64_t>(max_len, std::min<uint64_t>(p.in_len, p.bs));
+            small = small || p.in_len - (nb - 1) * p.bs <= 65536u;               // the last block is the shortest
+        }
+    }
+    if (out_cap < bound) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (nframes == 0) {
+        CTX_CUDA(ctx, cudaMemsetAsync(d_frame_off, 0, 8, s));
+        return LZ4B200_OK;
+    }
+    const uint32_t n = (uint32_t)nframes, nb = (uint32_t)nblocks;
+    CTX_CUDA(ctx, ctx->d_fplan.reserve(n));
+    CTX_CUDA(ctx, ctx->d_slots.reserve(slots + 16));
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve((size_t)nb + 1));
+    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb));
+    if (info->content_checksum) CTX_CUDA(ctx, ctx->d_content.reserve(n));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_fplan.p, plan.data(), n * sizeof(fb::FramePlan), cudaMemcpyHostToDevice, s));
+
+    const uint32_t bgrid = (nb + 127) / 128;
+    if (nb) {
+        frame_batch_blocks_kernel<<<bgrid, 128, 0, s>>>(ctx->d_fplan.p, n, nb, ctx->d_in_off.p, ctx->d_in_len.p,
+                                                        ctx->d_out_off.p, ctx->d_out_cap.p, ctx->d_flags.p,
+                                                        ctx->d_gdst.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+        // blocks on both sides of 64 KiB run both encoders whatever the bound says; an unknown bound (0) makes the
+        // launcher's record name both
+        const uint32_t max_in_len = small && max_len > 65536u ? 0u : (uint32_t)max_len;
+        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
+        const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
+        if (st != LZ4B200_OK) return st;
+        frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb,
+                                                                info->block_checksums ? 4u : 0u, ctx->d_info.p,
+                                                                ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);   // nb == 0: seg_off[0] = 0
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        frame_batch_dst_kernel<<<bgrid, 128, 0, s>>>(ctx->d_seg_off.p, nb, ctx->d_gdst.p);
+        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p, ctx->d_payload_len.p,
+                     ctx->d_pick.p, ctx->d_info.p, d_out, ctx->d_gdst.p, nb};
+        gather_segments_kernel<<<std::min<uint32_t>(std::max<uint32_t>(nb, (uint32_t)ctx->sm_count * 2),
+                                                    (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+        CTX_CUDA(ctx, cudaGetLastError());
+        if (info->block_checksums) {
+            frame_block_checksum_kernel<<<bgrid, 128, 0, s>>>(d_out, ctx->d_gdst.p, ctx->d_payload_len.p, nb);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    if (info->content_checksum) {
+        frame_batch_content_kernel<<<n, 256, 0, s>>>(d_in, ctx->d_fplan.p, ctx->d_content.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    frame_batch_tail_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_out, ctx->d_fplan.p, n, ctx->d_seg_off.p,
+                                                            info->content_checksum ? ctx->d_content.p : nullptr,
+                                                            d_frame_off);
     CTX_CUDA(ctx, cudaGetLastError());
     return LZ4B200_OK;
 }

@@ -1,0 +1,100 @@
+// lz4b200_frame_batch.cuh — the plan of the batch frame encoder (lz4b200_frame_compress_batch_device), shared by the
+// host and the device.
+//
+// The host plans every frame of a batch in one pass (plan_frame) and uploads the table.  The blocks of all frames are
+// numbered frame after frame and compressed in one launch; one GPU thread per block finds its frame by binary search
+// over the frames' first block indices and derives its input range, its scratch slot, its parse mode and where its
+// [BlockInfo | payload (| checksum)] segment lands in the packed output (batch_block).  Frames lie back to back: frame
+// f starts at seg_off[first_block] + ovh, where seg_off is the exclusive scan of every block's segment size and ovh the
+// header, EndMark and digest bytes of the frames before it (frame_place).
+// The header also compiles for the host alone (tests/cpp/frame_batch_host.cpp) for the CPU tests.
+#pragma once
+#include "lz4b200_frame_walk.cuh"
+
+namespace lz4b200 {
+namespace fb {
+
+// One frame of the batch, 64 bytes.
+struct FramePlan {
+    uint64_t in_off, in_len;       // the frame's input: d_in[in_off, in_off + in_len)
+    uint64_t slot_base;            // scratch bytes of the blocks of the frames before
+    uint64_t ovh;                  // header, EndMark and digest bytes of the frames before
+    uint32_t first_block;          // batch index of the frame's block 0
+    uint32_t bs;                   // the frame's block size
+    uint32_t fresh;                // table epoch: block k of the frame is FRESH iff k % fresh == 0 (frame/compress.rs:266-271)
+    uint8_t hdr[15];               // FrameInfo::write (header.rs:232-275): at most 15 bytes without a dictionary id
+    uint8_t hdr_len;
+    uint32_t pad;
+};
+
+// The scratch slot of a block of `len` input bytes: lz4b200_max_output_size(len) rounded up to 16 bytes.
+FW_FN uint64_t slot_bytes_for(uint64_t len) { return (20ull + len * 110ull / 100ull + 15ull) & ~15ull; }
+
+FW_FN uint64_t frame_blocks(const FramePlan &p) { return (p.in_len + p.bs - 1) / p.bs; }
+
+// Scratch of a frame: a slot per full block, and one sized for the last block's length.
+FW_FN uint64_t frame_slot_bytes(const FramePlan &p)
+{
+    const uint64_t nb = frame_blocks(p);
+    return nb ? (nb - 1) * slot_bytes_for(p.bs) + slot_bytes_for(p.in_len - (nb - 1) * p.bs) : 0;
+}
+
+// Completes p, whose input, block size, table period and header are set, from the frame before it (null: p is the
+// first).  `tail_len` is the EndMark and digest bytes every frame of the batch ends with (4, or 8 with a content
+// checksum).  The caller checks that the batch's blocks fit first_block.
+FW_FN void plan_frame(FramePlan &p, const FramePlan *prev, uint32_t tail_len)
+{
+    p.first_block = prev ? prev->first_block + (uint32_t)frame_blocks(*prev) : 0u;
+    p.slot_base = prev ? prev->slot_base + frame_slot_bytes(*prev) : 0u;
+    p.ovh = prev ? prev->ovh + prev->hdr_len + tail_len : 0u;
+}
+
+// The frame that holds batch block b: the last frame whose first block is at or before b (frames without blocks share
+// their successor's first block and come before it).
+FW_FN uint32_t find_frame(const FramePlan *p, uint32_t nframes, uint32_t b)
+{
+    uint32_t lo = 0, hi = nframes;                   // p[lo].first_block <= b, and b < p[hi].first_block or hi == nframes
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (p[mid].first_block <= b) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// What the compressor, the pack and the block checksums need of batch block b.
+struct BlockJob {
+    uint64_t in_off;               // input at d_in + in_off
+    uint64_t out_off;              // scratch slot
+    uint64_t dst_shift;            // the packed segment lands at seg_off[b] + dst_shift
+    uint32_t in_len, out_cap;
+    uint32_t frame, k;             // frame and frame-local index
+    uint8_t flags;                 // LZ4B200_BLOCK_* parse mode
+};
+
+FW_FN BlockJob batch_block(const FramePlan *p, uint32_t nframes, uint32_t b)
+{
+    BlockJob j;
+    j.frame = find_frame(p, nframes, b);
+    const FramePlan &q = p[j.frame];
+    j.k = b - q.first_block;
+    const uint64_t o = (uint64_t)j.k * q.bs, rem = q.in_len - o;
+    j.in_off = q.in_off + o;
+    j.in_len = (uint32_t)(rem < q.bs ? rem : q.bs);
+    j.out_off = q.slot_base + (uint64_t)j.k * slot_bytes_for(q.bs);
+    j.out_cap = (uint32_t)slot_bytes_for(j.in_len);
+    j.dst_shift = q.ovh + q.hdr_len;
+    j.flags = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (j.k % q.fresh == 0 ? 0u : LZ4B200_BLOCK_CONT));
+    return j;
+}
+
+// Where frame p lies in the packed output, given the scan of the segment sizes: its header at *start, its EndMark at
+// *endmark (the digest, when there is one, follows it).
+FW_FN void frame_place(const FramePlan &p, const uint64_t *seg_off, uint64_t *start, uint64_t *endmark)
+{
+    *start = seg_off[p.first_block] + p.ovh;
+    *endmark = seg_off[p.first_block + frame_blocks(p)] + p.ovh + p.hdr_len;
+}
+
+}  // namespace fb
+}  // namespace lz4b200

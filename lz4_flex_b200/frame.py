@@ -155,6 +155,65 @@ def compress_frame_device(d_in, frame_info: FrameInfo | None = None, out=None, c
     return out[:w]
 
 
+def _host_i64(v, what: str) -> np.ndarray:
+    if hasattr(v, "is_cuda"):
+        v = v.cpu().numpy()
+    a = np.ascontiguousarray(v, dtype=np.int64)
+    if a.ndim != 1:
+        raise TypeError(f"{what} must be 1-D")
+    if a.size and a.min() < 0:
+        raise ValueError(f"{what} must not be negative")
+    return a
+
+
+def compress_frames_device(d_in, offsets, lengths, frame_info: FrameInfo | None = None, out=None,
+                           ctx: _block.Context | None = None, stream: int | None = None):
+    """compress_frame() for each of many inputs in device memory, in one call (lz4b200_frame_compress_batch_device):
+    input i is d_in[offsets[i]:offsets[i] + lengths[i]], and its frame is byte-identical to what compress_frame() gives
+    for those bytes.  The frames are written back to back into `out` (a contiguous 1-D torch CUDA uint8 tensor; None:
+    one of the summed lz4b200_frame_bound bytes is allocated).  offsets and lengths are int64 sequences or arrays (a
+    CUDA tensor is copied to the host first).  frame_info is shared by every frame; BlockSize.Auto picks each frame's
+    block size from its own length, and a non-None content_size means "each frame records its own length" (the value
+    itself is ignored).  The work runs on torch's current stream (or `stream`); the call returns once the total length
+    has been read back.  Returns (view of `out` that holds the frames, CUDA int64 tensor of len(offsets) + 1 frame
+    offsets: frame i is out[frame_offsets[i]:frame_offsets[i + 1]]).  Raises what compress_frame() raises."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    info = frame_info or FrameInfo()
+    if info.block_mode == BlockMode.Linked:
+        raise LinkedBlocksUnsupported()
+    offs, lens = _host_i64(offsets, "offsets"), _host_i64(lengths, "lengths")
+    n = offs.size
+    if lens.size != n:
+        raise ValueError("offsets and lengths differ in length")
+    if n and int((offs + lens).max()) > d_in.numel():
+        raise ValueError("an input runs past the end of d_in")
+    ci = info.to_c()
+    if out is None:
+        # the sum of lz4b200_frame_bound over the frames, each with its resolved block size
+        if info.block_size == BlockSize.Auto:
+            bs = np.where(lens > 256 << 10, 4 << 20, np.where(lens > 64 << 10, 256 << 10, 64 << 10))
+        else:
+            bs = np.full(n, info.block_size.get_size(), dtype=np.int64)
+        total = int((27 + lens + 8 * ((lens + bs - 1) // bs)).sum()) if n else 0
+        out = torch.empty(total, dtype=torch.uint8, device=d_in.device)
+    _device_u8(out, "out")
+    s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+    frame_offsets = torch.empty(n + 1, dtype=torch.int64, device=out.device)
+    st = _native.lib().lz4b200_frame_compress_batch_device(
+        ctx.handle, d_in.data_ptr() if d_in.numel() else None, offs.ctypes.data, lens.ctypes.data, C.byref(ci),
+        out.data_ptr() if out.numel() else None, out.numel(), frame_offsets.data_ptr(), n, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    if stream is None:
+        total = int(frame_offsets[n].item())
+    else:
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=out.device)):
+            total = int(frame_offsets[n].item())                              # copied and synchronised on `stream`
+    return out[:total], frame_offsets
+
+
 def decompress_next_frame(data, ctx: _block.Context | None = None):
     """The frame that starts at data[0], through lz4b200_frame_decompress_next: returns
     (decoded bytes, consumed input bytes, exception or None).  Bytes decoded before an error are returned with it.
