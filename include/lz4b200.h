@@ -415,6 +415,61 @@ lz4b200_status lz4b200_frame_decoded_bound_batch_device(lz4b200_ctx *ctx,
     const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
     uint64_t *d_bound, size_t nframes, void *stream);
 
+/* Streaming frame decoder over DEVICE memory: FrameDecoder (frame/decompress.rs:109-342), which reads a frame one
+ * block at a time, for compressed bytes that arrive in HBM chunk by chunk (a GPUDirect Storage reader, a network
+ * receive) and decoded output taken in caller-sized pieces.  Its device memory does not depend on the frame's length:
+ * the context's frame budget (slots and staged payload), the caller's buffers, and the decoder's own 128 KiB (a linked
+ * frame's 64 KiB window, double-buffered) and hash state.  Linked frames (what `lz4`, LZ4F and pyarrow write by
+ * default) cross calls and groups through the window.  Linked decoding is still one serial chain per frame.
+ * A decoder belongs to one context; destroy it before the context.  Its persistent state (walk position, header
+ * fields, output so far, window, content hash) is its own; descriptors, slots and staged payload are the context's
+ * scratch, so other calls on the context, another decoder's included, may run between two of its calls, ordered on
+ * one stream as every device call of a context is. */
+typedef struct lz4b200_frame_decoder lz4b200_frame_decoder;
+lz4b200_status lz4b200_frame_decoder_create(lz4b200_ctx *ctx, lz4b200_frame_decoder **out);
+void lz4b200_frame_decoder_destroy(lz4b200_frame_decoder *dec);
+
+typedef struct lz4b200_frame_decoder_step {
+    uint64_t consumed;            /* bytes of d_in this call used: whole units only */
+    uint64_t written;             /* d_out[0, written) was written; nothing past it */
+    uint64_t need;                /* stopped for lack of input: at least this many bytes from d_in + consumed make the
+                                     next unit; else 0 */
+    int32_t frame_done;           /* 1: the frame ended in this call, and `result` is its result */
+    int32_t pad;
+    lz4b200_frame_result result;  /* the frame's result as lz4b200_frame_decompress_next returns it (below) */
+} lz4b200_frame_decoder_step;     /* 72 bytes */
+
+/* Continues the frame in progress with d_in[0, n), or starts one at d_in[0]; decodes into d_out[0, out_cap).
+ *   - input: a call takes whole units only (the header; a block: BlockInfo, payload and block checksum; the EndMark
+ *     with the content checksum).  The caller presents the unconsumed rest again, with more bytes after it.  With
+ *     end_of_input == 0, running out of input is never an error: the call stops and sets `need`.  With end_of_input
+ *     set, d_in runs to the end of the input, and a truncated unit ends the frame as _next reports it.
+ *   - output: the call decodes consecutive whole blocks while the sum of their decoded bounds (min(block size,
+ *     255 x payload); a stored block its length) fits out_cap, and while the group loop would not cut them (their slots
+ *     and input span fit the frame budget).  At most 65 536 blocks per call: a call may stop with need == 0 and input
+ *     left, and the caller calls again.  When the next block's bound alone exceeds out_cap the call returns
+ *     LZ4B200_FRAME_OUTPUT_FULL having consumed nothing, and the decoder is as it was.  An out_cap of at least the
+ *     frame's block size (8 MiB for legacy frames) always makes progress.
+ *   - frames: a call never crosses a frame boundary.  When the frame ends (EndMark, an error, or the end of input),
+ *     frame_done = 1 and the next call starts a new frame, as the reference's reader returns Ok(0) at each EndMark.
+ *     At end_of_input with nothing left the result is _next's for empty input: OK, 0 consumed, 0 written.
+ *   - the result: over every chunking of a frame F (end_of_input on the last chunk) and every out_cap of at least
+ *     its block size, the concatenated `written` bytes are what lz4b200_frame_decompress_next(F, cap = decoded bound)
+ *     writes, and `result` holds its status, written (the frame's total), block_status, err_expected, err_actual and
+ *     consumed (the frame's total).  One exception: after a block decode error (FRAME_DECOMPRESSION_ERROR) _next's
+ *     consumed is where its whole-frame walk ended, while the decoder's is the end of the failing block and its
+ *     checksum, where the reference's reader stands at that point.  Errors keep stream order: a decode error in an
+ *     earlier block wins over a later block's checksum failure, which cuts the frame at that block.
+ *   - INVALID_ARGUMENT, before anything is enqueued: a null decoder or step, a null d_in with n > 0, a null d_out with
+ *     out_cap > 0.  d_in and d_out may have any alignment.  Work runs on `stream`, which the call synchronises before
+ *     it returns; `step` is host memory. */
+lz4b200_status lz4b200_frame_decoder_decode_device(lz4b200_frame_decoder *dec, const uint8_t *d_in, size_t n,
+                                                   int end_of_input, uint8_t *d_out, size_t out_cap,
+                                                   lz4b200_frame_decoder_step *step, void *stream);
+
+/* Device bytes the context holds now, its scratch included (a diagnostic). */
+size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx);
+
 /* XXH32 (twox-hash XxHash32, Cargo.toml:51) — used for header/block/content checksums.
  * The streaming form backs FrameEncoder's running content hash (frame/compress.rs:141,320). */
 uint32_t lz4b200_xxh32(const uint8_t *data, size_t n, uint32_t seed);

@@ -95,6 +95,16 @@ class FrameInfoC(C.Structure):
     ]
 
 
+class FrameResultC(C.Structure):
+    _fields_ = [("consumed", C.c_uint64), ("written", C.c_uint64), ("err_expected", C.c_uint64),
+                ("err_actual", C.c_uint64), ("status", C.c_int32), ("block_status", C.c_int32)]
+
+
+class FrameDecoderStepC(C.Structure):
+    _fields_ = [("consumed", C.c_uint64), ("written", C.c_uint64), ("need", C.c_uint64), ("frame_done", C.c_int32),
+                ("pad", C.c_int32), ("result", FrameResultC)]
+
+
 _lib = None
 
 _vp, _sz, _u32, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_int
@@ -153,6 +163,10 @@ SIGNATURES = {
     "lz4b200_frame_decompress_batch_device": (_i32, [_vp] * 8 + [_sz, _vp]),
     "lz4b200_frame_decoded_bound_batch_device": (_i32, [_vp] * 5 + [_sz, _vp]),
     "lz4b200_ctx_set_frame_budget": (None, [_vp, _sz]),
+    "lz4b200_ctx_device_bytes": (_sz, [_vp]),
+    "lz4b200_frame_decoder_create": (_i32, [_vp, C.POINTER(_vp)]),
+    "lz4b200_frame_decoder_destroy": (None, [_vp]),
+    "lz4b200_frame_decoder_decode_device": (_i32, [_vp, _vp, _sz, _i32, _vp, _sz, C.POINTER(FrameDecoderStepC), _vp]),
     "lz4b200_xxh32": (_u32, [_vp, _sz, _u32]),
     "lz4b200_xxh32_reset": (None, [_vp, _u32]),
     "lz4b200_xxh32_update": (None, [_vp, _vp, _sz]),

@@ -158,6 +158,29 @@ __global__ void frame_walk_kernel(const uint8_t *in, uint64_t n, fw::FrameWalk *
     if (blockIdx.x == 0 && threadIdx.x == 0) fw::frame_walk(in, n, *w, out, max_blocks);
 }
 
+// The streaming decoder's walk (lz4b200_frame_decoder): one thread runs fw::frame_walk_stream over the presented chunk.
+__global__ void frame_walk_stream_kernel(const uint8_t *in, uint64_t n, bool eof, fw::FrameWalk *w, fw::FrameBlockDesc *out,
+                                         uint32_t max_blocks, uint64_t *need)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0) fw::frame_walk_stream(in, n, eof, *w, out, max_blocks, need);
+}
+
+// A linked frame's window after a group: the last min(64 KiB, old_len + n) bytes of old[0, old_len) followed by
+// add[0, n) (the group's output), into dst, which overlaps neither.  The bytes come from wherever they lie, across any
+// block or group boundary.
+constexpr uint32_t kWindowBytes = 65536;
+__global__ void __launch_bounds__(256) window_update_kernel(const uint8_t *old, uint32_t old_len, const uint8_t *add,
+                                                            uint64_t n, uint8_t *dst)
+{
+    const uint64_t total = old_len + n;
+    const uint32_t keep = (uint32_t)min(total, (uint64_t)kWindowBytes);
+    const uint64_t from = total - keep;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < keep; i += gridDim.x * blockDim.x) {
+        const uint64_t p = from + i;
+        dst[i] = p < old_len ? old[p] : add[p - old_len];
+    }
+}
+
 // Block checksums of the blocks the last walk launch recorded (frame indices first .. w->nblocks - 1), one thread per
 // block running the serial XXH32 over its payload; *bad receives the lowest index that fails.
 __global__ void __launch_bounds__(128) block_checksum_kernel(const uint8_t *in, const fw::FrameBlockDesc *desc,
@@ -2316,10 +2339,15 @@ lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool d
 // `in` and `out` are host memory (each group's payload is staged to the device and its output copied back), or with
 // `device` device memory, read and written in place.  When the frame has a content checksum, `content` (host memory,
 // or device memory with `device`) is carried over each group's output.  *written: the bytes delivered.
+// A linked frame's blocks may continue one decoded earlier (the streaming decoder, device memory only): `window` holds
+// the last `window_len` (<= 64 KiB) bytes of the frame's output before blocks[0], and the linked kernel sees it as a
+// stored block ahead of the group, staged with the group's payload in one buffer.  On FRAME_DECOMPRESSION_ERROR,
+// *failed (if not null) receives the index of the block that failed.
 lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, uint8_t *out,
                                    size_t cap, const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks,
                                    lz4b200_xxh32_state *content, size_t *written, int *block_status,
-                                   uint64_t *err_expected, uint64_t *err_actual)
+                                   uint64_t *err_expected, uint64_t *err_actual, const uint8_t *window = nullptr,
+                                   uint32_t window_len = 0, uint32_t *failed = nullptr)
 {
     const uint32_t nb = (uint32_t)blocks.size();
     const uint64_t bs = w.bs;
@@ -2327,7 +2355,8 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
     *written = 0;
     if (!nb) return LZ4B200_OK;
     DeviceGuard guard(ctx->device);
-    const bool linked = w.linked && nb > 1;
+    const bool linked = w.linked && (nb > 1 || window_len > 0);
+    const uint32_t pre = linked && window_len ? 1 : 0;                   // the window's pseudo-block ahead of the group
     std::vector<uint64_t> h_in_off, h_slot_off, seg, h_soff;
     std::vector<uint32_t> h_in_len, h_cap, produced, h_first, h_slen;
     std::vector<uint8_t> h_pick;
@@ -2344,70 +2373,79 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
             slot_total += fw::slot_bytes(c);
             g1++;
         }
-        const uint32_t gn = g1 - g0;
+        const uint32_t gn = g1 - g0, gm = gn + pre;                      // the kernel's blocks: [window,] the group
         const uint64_t in_lo = blocks[g0].payload_off;
         const uint64_t in_bytes = blocks[g1 - 1].payload_off + fw::block_len(blocks[g1 - 1]) - in_lo;
-        h_in_off.assign(gn, 0); h_slot_off.assign(gn, 0); h_in_len.assign(gn, 0); h_cap.assign(gn, 0);
-        h_pick.assign(gn, 0); produced.assign(gn, 0); status.assign(gn, 0); expected.assign(gn, 0); seg.assign(gn + 1, 0);
+        const uint64_t shift = pre ? window_len : 0;                       // the payload's place in a staged buffer
+        h_in_off.assign(gm, 0); h_slot_off.assign(gm, 0); h_in_len.assign(gm, 0); h_cap.assign(gm, 0);
+        h_pick.assign(gm, 0); produced.assign(gn, 0); status.assign(gn, 0); expected.assign(gn, 0); seg.assign(gn + 1, 0);
+        if (pre) h_pick[0] = 1;
         uint64_t so = 0;
         for (uint32_t k = 0; k < gn; k++) {
             const fw::FrameBlockDesc &b = blocks[g0 + k];
             const bool stored = fw::block_stored(b);
-            h_in_off[k] = b.payload_off - in_lo;
-            h_in_len[k] = stored ? 0 : fw::block_len(b);                 // stored blocks are only gathered
-            h_pick[k] = stored ? 1 : 0;
-            h_slot_off[k] = so;
-            h_cap[k] = (uint32_t)fw::block_slot_cap(b, bs);
-            so += fw::slot_bytes(h_cap[k]);
+            const uint32_t i = pre + k;
+            h_in_off[i] = b.payload_off - in_lo + shift;
+            h_in_len[i] = stored ? 0 : fw::block_len(b);                 // stored blocks are only gathered
+            h_pick[i] = stored ? 1 : 0;
+            h_slot_off[i] = so;
+            h_cap[i] = (uint32_t)fw::block_slot_cap(b, bs);
+            so += fw::slot_bytes(h_cap[i]);
         }
         const uint8_t *src = in + in_lo;                                   // the group's payload on the device
-        if (!device) {
-            CTX_CUDA(ctx, ctx->d_in.reserve(in_bytes + 16));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in + in_lo, in_bytes, cudaMemcpyHostToDevice, s));
+        if (!device || pre) {
+            CTX_CUDA(ctx, ctx->d_in.reserve(shift + in_bytes + 16));
+            if (pre) {
+                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, window, window_len, cudaMemcpyDeviceToDevice, s));
+                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p + shift, in + in_lo, in_bytes, cudaMemcpyDeviceToDevice, s));
+            } else {
+                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in + in_lo, in_bytes, cudaMemcpyHostToDevice, s));
+            }
             src = ctx->d_in.p;
         }
         CTX_CUDA(ctx, ctx->d_slots.reserve(so + 16));
-        CTX_CUDA(ctx, ctx->d_in_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_in_len.reserve(gn));
-        CTX_CUDA(ctx, ctx->d_out_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(gn));
-        CTX_CUDA(ctx, ctx->d_out_len.reserve(gn)); CTX_CUDA(ctx, ctx->d_status.reserve(gn));
-        CTX_CUDA(ctx, ctx->d_expected.reserve(gn));
-        CTX_CUDA(ctx, ctx->d_pick.reserve(gn)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(gn + 1));
+        CTX_CUDA(ctx, ctx->d_in_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_in_len.reserve(gm));
+        CTX_CUDA(ctx, ctx->d_out_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(gm));
+        CTX_CUDA(ctx, ctx->d_out_len.reserve(gm)); CTX_CUDA(ctx, ctx->d_status.reserve(gm));
+        CTX_CUDA(ctx, ctx->d_expected.reserve(gm));
+        CTX_CUDA(ctx, ctx->d_pick.reserve(gm)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(gn + 1));
         CTX_CUDA(ctx, ctx->d_payload_len.reserve(gn));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, h_in_len.data(), gn * 4, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_off.p, h_slot_off.data(), gn * 8, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_cap.p, h_cap.data(), gn * 4, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_pick.p, h_pick.data(), gn, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), gm * 8, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, h_in_len.data(), gm * 4, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_off.p, h_slot_off.data(), gm * 8, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_cap.p, h_cap.data(), gm * 4, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_pick.p, h_pick.data(), gm, cudaMemcpyHostToDevice, s));
         BatchArgs a{src, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
-                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, gn, nullptr};
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, gm, nullptr};
         lz4b200_status st;
         if (linked) {
             // BlockMode::Linked (frame/decompress.rs:196-222): the blocks of a frame form a dependency chain; the
             // linked kernel resolves offsets that reach before a block in the outputs of its predecessors
-            h_first.assign(gn, 0); h_slen.assign(gn, 0); h_soff.assign(gn, 0);
+            h_first.assign(gm, 0); h_slen.assign(gm, 0); h_soff.assign(gm, 0);
+            if (pre) h_slen[0] = window_len;
             for (uint32_t k = 0; k < gn; k++) {
-                h_slen[k] = fw::block_stored(blocks[g0 + k]) ? fw::block_len(blocks[g0 + k]) : 0;
-                h_soff[k] = h_in_off[k];
+                h_slen[pre + k] = fw::block_stored(blocks[g0 + k]) ? fw::block_len(blocks[g0 + k]) : 0;
+                h_soff[pre + k] = h_in_off[pre + k];
             }
-            CTX_CUDA(ctx, ctx->d_link_first.reserve(gn)); CTX_CUDA(ctx, ctx->d_stored_len.reserve(gn));
-            CTX_CUDA(ctx, ctx->d_stored_off.reserve(gn)); CTX_CUDA(ctx, ctx->d_done.reserve(gn));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_link_first.p, h_first.data(), gn * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_len.p, h_slen.data(), gn * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_off.p, h_soff.data(), gn * 8, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_done.p, 0, gn * 4, s));
+            CTX_CUDA(ctx, ctx->d_link_first.reserve(gm)); CTX_CUDA(ctx, ctx->d_stored_len.reserve(gm));
+            CTX_CUDA(ctx, ctx->d_stored_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_done.reserve(gm));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_link_first.p, h_first.data(), gm * 4, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_len.p, h_slen.data(), gm * 4, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_off.p, h_soff.data(), gm * 8, cudaMemcpyHostToDevice, s));
+            CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_done.p, 0, gm * 4, s));
             a.link_first = ctx->d_link_first.p; a.stored_off = ctx->d_stored_off.p;
             a.stored_len = ctx->d_stored_len.p; a.done = ctx->d_done.p;
             a.tickets = ctx->d_tickets;
-            const uint32_t grid = std::min<uint32_t>((gn + 3) / 4, (uint32_t)ctx->sm_count * 8);
+            const uint32_t grid = std::min<uint32_t>((gm + 3) / 4, (uint32_t)ctx->sm_count * 8);
             lz4_decompress_blocks_linked<32><<<grid, 128, 0, s>>>(a);
             st = ctx->check(cudaGetLastError(), "linked decode launch") ? LZ4B200_OK : LZ4B200_CUDA_ERROR;
         } else {
             st = launch_decompress(ctx, a, s);
         }
         if (st != LZ4B200_OK) return st;
-        CTX_CUDA(ctx, cudaMemcpyAsync(produced.data(), ctx->d_out_len.p, gn * 4, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(status.data(), ctx->d_status.p, gn * 4, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(expected.data(), ctx->d_expected.p, gn * 8, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(produced.data(), ctx->d_out_len.p + pre, gn * 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(status.data(), ctx->d_status.p + pre, gn * 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(expected.data(), ctx->d_expected.p + pre, gn * 8, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaStreamSynchronize(s));
 
         // first failing block (stream order) wins over anything the walk found later
@@ -2428,8 +2466,8 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
             }
             CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_seg_off.p, seg.data(), (good + 1) * 8, cudaMemcpyHostToDevice, s));
             CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_payload_len.p, produced.data(), good * 4, cudaMemcpyHostToDevice, s));
-            GatherArgs g{ctx->d_slots.p, src, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p,
-                         ctx->d_payload_len.p, ctx->d_pick.p, nullptr, dst, ctx->d_seg_off.p, good};
+            GatherArgs g{ctx->d_slots.p, src, ctx->d_out_off.p + pre, ctx->d_in_off.p + pre, ctx->d_payload_len.p,
+                         ctx->d_payload_len.p, ctx->d_pick.p + pre, nullptr, dst, ctx->d_seg_off.p, good};
             gather_segments_kernel<<<std::min<uint32_t>(good, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
             CTX_CUDA(ctx, cudaGetLastError());
             if (device) {
@@ -2449,8 +2487,9 @@ lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device
             if (block_status) *block_status = status[good];
             if (status[good] == LZ4B200_DEC_OUTPUT_TOO_SMALL) {
                 if (err_expected) *err_expected = expected[good];
-                if (err_actual) *err_actual = h_cap[good];
+                if (err_actual) *err_actual = h_cap[pre + good];
             }
+            if (failed) *failed = g0 + good;
             return LZ4B200_FRAME_DECOMPRESSION_ERROR;
         }
         g0 = g1;
@@ -2751,6 +2790,227 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
         ip += used;
     }
     return LZ4B200_OK;
+}
+
+size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
+{
+    if (!ctx) return 0;
+    size_t b = ctx->d_tickets ? 8 * sizeof(uint32_t) : 0;
+    auto add = [&b](const auto &buf) { b += buf.cap * sizeof(*buf.p); };
+    add(ctx->d_gtab16);
+#ifdef LZ4B200_AB_VARIANTS
+    add(ctx->d_ttab16); add(ctx->d_gtag32);
+#endif
+    add(ctx->d_in); add(ctx->d_out); add(ctx->d_slots); add(ctx->d_flags); add(ctx->d_pick); add(ctx->d_dict);
+    add(ctx->d_in_off); add(ctx->d_out_off); add(ctx->d_seg_off); add(ctx->d_expected); add(ctx->d_off_b);
+    add(ctx->d_in_len); add(ctx->d_out_cap); add(ctx->d_out_len); add(ctx->d_info); add(ctx->d_seg_size);
+    add(ctx->d_payload_len); add(ctx->d_link_first); add(ctx->d_stored_len); add(ctx->d_done); add(ctx->d_stored_off);
+    add(ctx->d_status); add(ctx->d_walk); add(ctx->d_desc); add(ctx->d_bad); add(ctx->d_content);
+    add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_fbase); add(ctx->d_fbad); add(ctx->d_bframe);
+    add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
+    if (const Pipeline *p = static_cast<const Pipeline *>(ctx->pipe)) {
+        for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
+        if (p->d_tickets) b += kMaxLanes * 8 * sizeof(uint32_t);
+    }
+    return b;
+}
+
+// ---- streaming frame decoder (FrameDecoder over device memory, frame/decompress.rs:109-342) ------------------------------
+// The decoder holds what must outlive a call: the walk of the frame in progress, the frame's output so far, a linked
+// frame's window and the running content hash.  Descriptors, slots and staged payload are the context's scratch, so other
+// calls on the context may come between two of its calls.
+struct lz4b200_frame_decoder {
+    lz4b200_ctx *ctx = nullptr;
+    int device = 0;                           // the context's device (the decoder's buffers live there)
+    fw::FrameWalk w;                          // the frame in progress, offsets from its first byte (fresh: no frame yet)
+    uint64_t written = 0;                     // bytes the frame has decoded so far
+    uint32_t win_len = 0, win = 0;            // linked frames: bytes in the window, and which half of d_win holds them
+    DevBuf<uint8_t> d_win;                    // two halves of kWindowBytes: the window, and the next one
+    DevBuf<lz4b200_xxh32_state> d_content;    // the running content hash
+    DevBuf<uint64_t> d_need;                  // what the walk needs to go on
+};
+
+namespace {
+
+// The frame ends in this call with status `st` after `consumed` bytes; the decoder waits for the next frame.
+void decoder_finish(lz4b200_frame_decoder *dec, lz4b200_frame_decoder_step &step, lz4b200_status st, uint64_t consumed)
+{
+    step.frame_done = 1;
+    step.result.status = st;
+    step.result.consumed = consumed;
+    step.result.written = dec->written;
+    dec->w = fw::FrameWalk{};
+    dec->written = 0;
+    dec->win_len = 0;
+}
+
+// One call: walk the presented chunk, take the blocks that fit out_cap and the frame budget, check their checksums,
+// decode them as one group of the group loop, and carry the window and the content hash to the next call.
+lz4b200_status decoder_step(lz4b200_frame_decoder *dec, cudaStream_t s, const uint8_t *d_in, size_t n, bool eof,
+                            uint8_t *d_out, size_t out_cap, lz4b200_frame_decoder_step &step)
+{
+    lz4b200_ctx *ctx = dec->ctx;
+    const fw::FrameWalk w0 = dec->w;
+    const uint64_t at = w0.ip;                                    // the frame's bytes before d_in[0]
+    CTX_CUDA(ctx, ctx->d_walk.reserve(2)); CTX_CUDA(ctx, ctx->d_desc.reserve(kDeviceWalkChunk));
+    CTX_CUDA(ctx, ctx->d_bad.reserve(1));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p, &w0, sizeof w0, cudaMemcpyHostToDevice, s));
+    frame_walk_stream_kernel<<<1, 1, 0, s>>>(d_in, n, eof, ctx->d_walk.p, ctx->d_desc.p, kDeviceWalkChunk, dec->d_need.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    fw::FrameWalk w1;
+    uint64_t need = 0;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&w1, ctx->d_walk.p, sizeof w1, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(&need, dec->d_need.p, sizeof need, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    const uint32_t k = (uint32_t)(w1.nblocks - w0.nblocks);
+    std::vector<fw::FrameBlockDesc> blocks(k);                    // payload offsets from d_in[0]
+    if (k) {
+        CTX_CUDA(ctx, cudaMemcpyAsync(blocks.data(), ctx->d_desc.p, k * sizeof(fw::FrameBlockDesc), cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+
+    // the blocks this call decodes: the longest prefix whose decoded bounds fit out_cap and that the group loop would
+    // not cut (slots and input span within the frame budget)
+    uint32_t t = 0;
+    for (uint64_t bound = 0, slots = 0; t < k; t++) {
+        const fw::FrameBlockDesc &b = blocks[t];
+        const uint64_t cap = fw::block_slot_cap(b, w1.bs);
+        const uint64_t ob = fw::block_stored(b) ? fw::block_len(b) : cap;
+        if (bound + ob > out_cap) break;
+        if (t && fw::group_cut(slots, cap, b.payload_off + fw::block_len(b) - blocks[0].payload_off, ctx->frame_budget))
+            break;
+        bound += ob;
+        slots += fw::slot_bytes(cap);
+    }
+    if (k && !t) return LZ4B200_FRAME_OUTPUT_FULL;                // the next block alone does not fit: nothing is taken
+
+    // block checksums of the blocks taken: the first that fails ends the frame there
+    uint32_t bad = fw::kNoBlock;
+    if (t && (w1.flg & 0x10)) {
+        fw::FrameWalk wt = w1;
+        wt.nblocks = t;
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p + 1, &wt, sizeof wt, cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bad.p, 0xff, 4, s));
+        block_checksum_kernel<<<(t + 127) / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_walk.p + 1, 0, ctx->d_bad.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+        CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    }
+    fw::FrameWalk wn = w1;                                        // the walk as this call leaves it
+    if (bad < t) {
+        fw::frame_walk_fail_block(wn, blocks[bad], (uint32_t)(w0.nblocks + bad));
+        wn.ip += at;
+        wn.stage = fw::kWalkDone;
+        t = bad;
+    } else if (t < k) {
+        wn.ip = at + blocks[t].payload_off - 4;                   // at the BlockInfo of the first block not taken
+        wn.nblocks = w0.nblocks + t;
+        wn.stage = fw::kWalkBlocks;
+        wn.status = LZ4B200_OK;
+        wn.closed = wn.has_checksum = 0;
+        wn.content_checksum = 0;
+        need = 0;
+    }
+    if (w0.stage == fw::kWalkHeader) {
+        lz4b200_xxh32_state c;
+        fw::xxh32_reset(c, 0);
+        CTX_CUDA(ctx, cudaMemcpyAsync(dec->d_content.p, &c, sizeof c, cudaMemcpyHostToDevice, s));
+    }
+
+    blocks.resize(t);
+    fw::FrameWalk wd = wn;
+    wd.has_checksum = (wn.flg & 0x04) != 0;                       // hashed as groups land: the EndMark may come later
+    size_t got = 0;
+    int bstat = 0;
+    uint64_t e1 = 0, e2 = 0;
+    uint32_t failed = fw::kNoBlock;
+    const lz4b200_status st = decode_frame_blocks(ctx, s, true, d_in, d_out, out_cap, wd, blocks, dec->d_content.p, &got,
+                                                  &bstat, &e1, &e2, dec->d_win.p + (size_t)dec->win * kWindowBytes,
+                                                  dec->win_len, &failed);
+    if (st != LZ4B200_OK && st != LZ4B200_FRAME_DECOMPRESSION_ERROR) return st;
+    dec->written += got;
+    step.written = got;
+    if (st == LZ4B200_FRAME_DECOMPRESSION_ERROR) {
+        // the reference's reader stands after the failing block and its checksum
+        const fw::FrameBlockDesc &b = blocks[failed];
+        step.consumed = b.payload_off + fw::block_len(b) + ((wn.flg & 0x10) ? 4 : 0);
+        step.result.block_status = bstat;
+        step.result.err_expected = e1;
+        step.result.err_actual = e2;
+        decoder_finish(dec, step, st, at + step.consumed);
+        return LZ4B200_OK;
+    }
+    step.consumed = wn.ip - at;
+    if (wn.stage == fw::kWalkDone) {
+        // content size and checksum at the EndMark (decompress.rs:312-331)
+        lz4b200_status fs = (lz4b200_status)wn.status;
+        if (fs == LZ4B200_OK && wn.closed) {
+            if (wn.has_size && dec->written != wn.content_size) {
+                fs = LZ4B200_FRAME_CONTENT_LENGTH;
+                step.result.err_expected = wn.content_size;
+                step.result.err_actual = dec->written;
+            } else if (wn.has_checksum) {
+                lz4b200_xxh32_state c;
+                CTX_CUDA(ctx, cudaMemcpyAsync(&c, dec->d_content.p, sizeof c, cudaMemcpyDeviceToHost, s));
+                CTX_CUDA(ctx, cudaStreamSynchronize(s));
+                if (fw::xxh32_digest(c) != wn.content_checksum) fs = LZ4B200_FRAME_CONTENT_CHECKSUM;
+            }
+        }
+        decoder_finish(dec, step, fs, wn.ip);
+        return LZ4B200_OK;
+    }
+    if (wn.linked && got) {
+        uint8_t *old = dec->d_win.p + (size_t)dec->win * kWindowBytes;
+        uint8_t *next = dec->d_win.p + (size_t)(dec->win ^ 1) * kWindowBytes;
+        window_update_kernel<<<64, 256, 0, s>>>(old, dec->win_len, d_out, got, next);
+        CTX_CUDA(ctx, cudaGetLastError());
+        dec->win ^= 1;
+        dec->win_len = (uint32_t)std::min<uint64_t>(kWindowBytes, dec->win_len + got);
+    }
+    dec->w = wn;
+    step.need = need;
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+lz4b200_status lz4b200_frame_decoder_create(lz4b200_ctx *ctx, lz4b200_frame_decoder **out)
+{
+    if (!ctx || !out) return LZ4B200_INVALID_ARGUMENT;
+    *out = nullptr;
+    DeviceGuard guard(ctx->device);
+    lz4b200_frame_decoder *dec = new lz4b200_frame_decoder();
+    dec->ctx = ctx;
+    dec->device = ctx->device;
+    if (!ctx->check(dec->d_win.reserve(2 * kWindowBytes), "decoder window") ||
+        !ctx->check(dec->d_content.reserve(1), "decoder content hash") || !ctx->check(dec->d_need.reserve(1), "decoder need")) {
+        lz4b200_frame_decoder_destroy(dec);
+        return LZ4B200_CUDA_ERROR;
+    }
+    *out = dec;
+    return LZ4B200_OK;
+}
+
+void lz4b200_frame_decoder_destroy(lz4b200_frame_decoder *dec)
+{
+    if (!dec) return;
+    DeviceGuard guard(dec->device);
+    dec->d_win.release(); dec->d_content.release(); dec->d_need.release();
+    delete dec;
+}
+
+lz4b200_status lz4b200_frame_decoder_decode_device(lz4b200_frame_decoder *dec, const uint8_t *d_in, size_t n,
+                                                   int end_of_input, uint8_t *d_out, size_t out_cap,
+                                                   lz4b200_frame_decoder_step *step, void *stream)
+{
+    if (!dec || !step || (!d_in && n) || (!d_out && out_cap)) return LZ4B200_INVALID_ARGUMENT;
+    *step = lz4b200_frame_decoder_step{};
+    lz4b200_ctx *ctx = dec->ctx;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const lz4b200_status st = decoder_step(dec, s, d_in, n, end_of_input != 0, d_out, out_cap, *step);
+    if (st != LZ4B200_CUDA_ERROR) CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    return st;
 }
 
 }  // extern "C"

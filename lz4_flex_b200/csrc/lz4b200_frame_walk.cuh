@@ -188,6 +188,54 @@ FW_FN uint32_t frame_walk(const uint8_t *in, uint64_t n, FrameWalk &w, FrameBloc
     return k;
 }
 
+// ---- the walk over a frame that arrives in chunks (lz4b200_frame_decoder) ---------------------------------------------
+// Bytes the unit at p[0, avail) takes: the header, a block (BlockInfo, payload, block checksum) or the EndMark with the
+// content checksum.  While p[] is too short to tell, the bytes that tell more (4, then 7 for a header); a unit the walk
+// rejects from its first bytes (a bad magic, BlockTooBig) takes no more than those.
+FW_FN uint64_t walk_unit_bytes(const uint8_t *p, uint64_t avail, const FrameWalk &w)
+{
+    if (avail < 4) return 4;
+    if (w.stage == kWalkHeader) {
+        const uint32_t magic = rd32(p);
+        if (magic == 0x184C2102u) return 4;
+        if (avail < 7 || magic != 0x184D2204u) return 7;
+        return 7 + ((p[4] & 0x08) ? 8 : 0) + ((p[4] & 0x01) ? 4 : 0);
+    }
+    const uint32_t word = rd32(p);
+    if (word == 0) return 4 + ((w.flg & 0x04) ? 4 : 0);
+    const uint64_t len = word & 0x7fffffffu;
+    if (len > w.bs) return 4;
+    return 4 + len + ((w.flg & 0x10) ? 4 : 0);
+}
+
+// frame_walk over a frame presented in chunks.  in[0, n) holds the frame's bytes from w.ip on: a call starts where the
+// last one stopped, and w.ip stays an offset from the frame's first byte.  Recorded payload offsets are from in[0].  It
+// takes whole units only, at most max_blocks blocks.  Unless `eof` (in[0, n) runs to the end of the input), it stops
+// before a unit in[] does not hold whole, with no status set, and *need receives the bytes from that unit's start it
+// needs at least; otherwise *need = 0.  With `eof` a truncated unit ends the walk as frame_walk ends it.  So any
+// chunking of a frame, `eof` on the last chunk, records the blocks frame_walk records and leaves the same FrameWalk.
+// It never reads at or past n.
+FW_FN uint32_t frame_walk_stream(const uint8_t *in, uint64_t n, bool eof, FrameWalk &w, FrameBlockDesc *out,
+                                 uint32_t max_blocks, uint64_t *need)
+{
+    const uint64_t at = w.ip;
+    uint32_t k = 0;
+    *need = 0;
+    while (w.stage != kWalkDone && k < max_blocks) {
+        const uint64_t rel = w.ip - at;
+        const uint64_t unit = walk_unit_bytes(in + rel, n - rel, w);
+        if (!eof && unit > n - rel) { *need = unit; break; }
+        const uint64_t lim = eof ? n : rel + unit;
+        if (w.stage == kWalkHeader) { walk_header(in, lim, w); continue; }   // only ever at the frame's first byte
+        FrameWalk u = w;
+        u.ip = rel;
+        k += frame_walk(in, lim, u, out + k, 1);
+        u.ip += at;
+        w = u;
+    }
+    return k;
+}
+
 // The block checksum (frame/decompress.rs:258-266): XXH32 of the payload as stored.
 FW_FN bool block_checksum_ok(const uint8_t *in, const FrameBlockDesc &b)
 {

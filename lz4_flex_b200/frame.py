@@ -401,6 +401,90 @@ def decompress_frames_device(d_in, offsets, lengths, out=None, out_offsets=None,
     return DecodedFrames(out, oo, results)
 
 
+class DeviceFrameDecoder:
+    """FrameDecoder over device memory (lz4b200_frame_decoder): decodes frames whose compressed bytes arrive in device
+    memory chunk by chunk, into caller-sized output pieces, in device memory that does not grow with the frame (the
+    context's frame budget and a 64 KiB window).  Linked frames included."""
+
+    def __init__(self, ctx: _block.Context | None = None):
+        self.ctx = ctx or _block.default_context()
+        h = C.c_void_p()
+        st = _native.lib().lz4b200_frame_decoder_create(self.ctx.handle, C.byref(h))
+        if st != 0:
+            raise error_from_status(st, detail=self.ctx.last_cuda_error())
+        self._h = h
+
+    def close(self):
+        if self._h:
+            _native.lib().lz4b200_frame_decoder_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def decode(self, d_in, d_out, end_of_input: bool = False, stream: int | None = None):
+        """Continues the frame in progress with d_in (or starts one at d_in[0]) and decodes into d_out; both are
+        contiguous 1-D torch CUDA uint8 tensors.  Returns (consumed, written, need, done, err): the whole units of d_in
+        used, the bytes of d_out written, the bytes from d_in[consumed] the next unit needs when the call stopped for
+        input (else 0), whether the frame ended, and then the exception decompress_next_frame_device() would raise for
+        it (or None).  Present the unconsumed rest of d_in again with more bytes after it; set end_of_input when d_in
+        runs to the end of the input.  Raises IoError when d_out cannot hold the next block (nothing is consumed).
+        The work runs on torch's current stream (or `stream`) and the call returns once d_out holds the result."""
+        import torch
+        _device_u8(d_in, "d_in")
+        _device_u8(d_out, "d_out")
+        s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+        n, cap = d_in.numel(), d_out.numel()
+        step = _native.FrameDecoderStepC()
+        st = _native.lib().lz4b200_frame_decoder_decode_device(self._h, d_in.data_ptr() if n else None, n,
+                                                                1 if end_of_input else 0,
+                                                                d_out.data_ptr() if cap else None, cap, C.byref(step), s)
+        if st != 0:
+            raise error_from_status(st, detail=self.ctx.last_cuda_error())
+        r = step.result
+        err = None
+        if step.frame_done and r.status != 0:
+            err = error_from_status(r.status, r.block_status, self.ctx.last_cuda_error(), r.err_expected, r.err_actual)
+        return step.consumed, step.written, step.need, bool(step.frame_done), err
+
+
+def iter_decompress_device(read_into, out_bytes: int = 8 << 20, in_bytes: int = 16 << 20, ctx: _block.Context | None = None,
+                           device=None):
+    """Every concatenated frame of a compressed stream that arrives in device memory, decoded in bounded device memory.
+    read_into(buf) writes the next compressed bytes to the start of the device tensor `buf` and returns how many (0 at
+    the end of the input).  Yields (view, frame_done): views of an output buffer of out_bytes (at least the frames'
+    block size: 8 MiB covers every frame), each valid until the next item is taken; frame_done marks a frame's last
+    piece.  Raises what decompress_frame_device() raises, after yielding the bytes decoded before the error.  Compressed
+    units must fit in_bytes (a 4 MiB block takes 4 MiB + 8 bytes)."""
+    import torch
+    dec = DeviceFrameDecoder(ctx)
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    buf = torch.empty(in_bytes, dtype=torch.uint8, device=dev)
+    out = torch.empty(out_bytes, dtype=torch.uint8, device=dev)
+    pos, have, eof = 0, 0, False
+    try:
+        while True:
+            if not eof and (pos or have < in_bytes):
+                if pos:
+                    buf[:have - pos] = buf[pos:have].clone()
+                    have, pos = have - pos, 0
+                got = int(read_into(buf[have:]))
+                eof = got == 0
+                have += got
+            consumed, written, need, done, err = dec.decode(buf[pos:have], out, end_of_input=eof)
+            if done and consumed == 0 and written == 0 and err is None:
+                return                                                     # end of data: nothing left to decode
+            if written or done:
+                yield out[:written], done
+            if err is not None:
+                raise err
+            pos += consumed
+            if need and pos == 0 and have == in_bytes:
+                raise ValueError(f"a compressed unit of {need} bytes does not fit in_bytes={in_bytes}")
+    finally:
+        dec.close()
+
+
 # -----------------------------------------------------------------------------------------------------
 # FrameEncoder
 # -----------------------------------------------------------------------------------------------------
