@@ -357,7 +357,10 @@ size_t lz4b200_frame_write_header(const lz4b200_frame_info *info, uint8_t *out, 
  *     default) are decoded too: their blocks form a dependency chain that the device resolves in stream order;
  *   - device memory is bounded: independent blocks are decoded in groups whose output slots
  *     (min(block size, 255 x payload) each) fit lz4b200_ctx_set_frame_budget() bytes (default 256 MiB), reusing the
- *     slots from group to group — the reference decodes any frame in O(block size) memory. */
+ *     slots from group to group — the reference decodes any frame in O(block size) memory.
+ * lz4b200_ctx_set_frame_budget (at least 1 MiB) bounds the device memory of the frame decoders and of the streaming
+ * frame encoder (lz4b200_frame_encoder, below): per group, the decoders' slots and staged input, and the encoder's
+ * buffered input and slots. */
 lz4b200_status lz4b200_frame_decompress_next(lz4b200_ctx *ctx, const uint8_t *in, size_t n,
                                              uint8_t *out, size_t cap, size_t *consumed, size_t *written,
                                              int *block_status, uint64_t *err_expected, uint64_t *err_actual);
@@ -466,6 +469,66 @@ typedef struct lz4b200_frame_decoder_step {
 lz4b200_status lz4b200_frame_decoder_decode_device(lz4b200_frame_decoder *dec, const uint8_t *d_in, size_t n,
                                                    int end_of_input, uint8_t *d_out, size_t out_cap,
                                                    lz4b200_frame_decoder_step *step, void *stream);
+
+/* Streaming frame encoder over DEVICE memory: FrameEncoder (frame/compress.rs:62-404), an io::Write over any number of
+ * write_all, flush and try_finish calls, for input that a GPU producer writes in pieces (a checkpoint writer, a
+ * GPUDirect Storage writer, a simulation dumping fields) or that is too large to be resident at once.  Its device
+ * memory does not depend on the stream's length or on a call's length: one input buffer of a group of whole blocks,
+ * the context's slots and descriptors for that group, and about 14 KiB of its own (hash state and output position).
+ * A group is as many blocks as fit the context's frame budget (lz4b200_ctx_set_frame_budget), each counting its block
+ * size of buffer and its lz4b200_max_output_size(block size) slot; at least one block.  At the default 256 MiB budget a
+ * group of 64 KiB blocks is 1 950 blocks.  The buffer is (re)allocated when a frame opens, the point where BlockSize
+ * Auto resolves, and only when the block size or the budget has changed; a frame keeps its group to its end.
+ * An encoder belongs to one context; destroy it before the context.  Its state is its own; descriptors and slots are
+ * the context's scratch, so other calls on the context, another encoder's or a decoder's included, may run between two
+ * of its calls, ordered on one stream as every device call of a context is.
+ * create: INVALID_ARGUMENT for a null ctx, info or out, or a block size id other than 0 or 4..7;
+ * FRAME_LINKED_UNSUPPORTED for linked blocks. */
+typedef struct lz4b200_frame_encoder lz4b200_frame_encoder;
+lz4b200_status lz4b200_frame_encoder_create(lz4b200_ctx *ctx, const lz4b200_frame_info *info,
+                                            lz4b200_frame_encoder **out);
+void lz4b200_frame_encoder_destroy(lz4b200_frame_encoder *enc);
+
+#define LZ4B200_ENCODE_WRITE  0   /* write_all(d_in)                 */
+#define LZ4B200_ENCODE_FLUSH  1   /* write_all(d_in); flush()        */
+#define LZ4B200_ENCODE_FINISH 2   /* write_all(d_in); try_finish()   */
+
+/* The most bytes lz4b200_frame_encoder_encode_device(enc, ., n, op, ...) can write in the encoder's current state: the
+ * header when the call opens a frame, 4 + length (+ 4 with block checksums) for every block of every group the call
+ * completes, and for FINISH the EndMark (+ 4 with a content checksum).  0 for a null encoder or an unknown op. */
+size_t lz4b200_frame_encoder_bound(const lz4b200_frame_encoder *enc, size_t n, int op);
+
+/* content_len of the open (or last) frame: the input bytes it has taken so far.  With a FRAME_CONTENT_LENGTH result it
+ * is the `actual` of ContentLengthError{expected, actual}. */
+uint64_t lz4b200_frame_encoder_content_len(const lz4b200_frame_encoder *enc);
+
+/* write_all(d_in[0, n)), then flush() (FLUSH) or try_finish() (FINISH), writing the call's bytes to d_out[0, *d_written).
+ *   - output: over any sequence of calls on one encoder (empty writes, flushes, finishes, writes after a finish, which
+ *     open the next frame), the concatenated d_out[0, *d_written) of the calls are what lz4_flex's FrameEncoder writes
+ *     for the same sequence of write_all / flush / try_finish, quirks included: Auto resolves from the first non-empty
+ *     write of the first frame and stays resolved for later frames; FINISH with nothing written writes an empty frame
+ *     (header and EndMark); a second FINISH writes a second EndMark (and the last frame's digest); the stream state is
+ *     reset when a frame opens after a frame that had content.  Only when the bytes appear differs: input is buffered
+ *     and compressed in whole groups.  Bytes of d_out past *d_written are not written.
+ *   - buffering: the input is copied into the encoder's buffer; each time it holds a full group, the group is
+ *     compressed and the buffer empties.  FLUSH and FINISH compress what is buffered, the last block short.  The caller
+ *     may reuse d_in once `stream` has passed the call.  Each block's parse mode follows the stream offset
+ *     (compress.rs:266-271, 357-367), planned on the host; after a flush it is not the block index's.
+ *   - the groups of a call pack back to back after the header, which is written only when the call opens a frame.  Block
+ *     checksums are computed one GPU thread per block; the content hash runs over each group's input in stream order and
+ *     is finished by the kernel that writes the EndMark.
+ *   - errors, reported before anything is enqueued, the encoder, d_out and *d_written untouched, in this order:
+ *       INVALID_ARGUMENT           a null encoder or d_written, a null d_out with out_cap > 0; a null d_in with n > 0;
+ *                                  an op other than LZ4B200_ENCODE_WRITE, _FLUSH or _FINISH;
+ *       COMPRESS_OUTPUT_TOO_SMALL  out_cap < lz4b200_frame_encoder_bound(enc, n, op).
+ *   - FINISH when the frame records a content size other than its content_len behaves as try_finish does
+ *     (compress.rs:209-219): the flushed blocks are written and counted in *d_written, no EndMark is written, the frame
+ *     is closed and the call returns FRAME_CONTENT_LENGTH.
+ *   - the work is enqueued on `stream` and the call returns without synchronising; *d_written is a device u64.  Only
+ *     kernel arguments and each group's parse modes cross PCIe.  d_in and d_out may have any alignment and must not
+ *     overlap. */
+lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, const uint8_t *d_in, size_t n, int op,
+                                                   uint8_t *d_out, size_t out_cap, uint64_t *d_written, void *stream);
 
 /* Device bytes the context holds now, its scratch included (a diagnostic). */
 size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx);

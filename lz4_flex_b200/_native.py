@@ -167,6 +167,11 @@ SIGNATURES = {
     "lz4b200_frame_decoder_create": (_i32, [_vp, C.POINTER(_vp)]),
     "lz4b200_frame_decoder_destroy": (None, [_vp]),
     "lz4b200_frame_decoder_decode_device": (_i32, [_vp, _vp, _sz, _i32, _vp, _sz, C.POINTER(FrameDecoderStepC), _vp]),
+    "lz4b200_frame_encoder_create": (_i32, [_vp, C.POINTER(FrameInfoC), C.POINTER(_vp)]),
+    "lz4b200_frame_encoder_destroy": (None, [_vp]),
+    "lz4b200_frame_encoder_bound": (_sz, [_vp, _sz, _i32]),
+    "lz4b200_frame_encoder_content_len": (C.c_uint64, [_vp]),
+    "lz4b200_frame_encoder_encode_device": (_i32, [_vp, _vp, _sz, _i32, _vp, _sz, _vp, _vp]),
     "lz4b200_xxh32": (_u32, [_vp, _sz, _u32]),
     "lz4b200_xxh32_reset": (None, [_vp, _u32]),
     "lz4b200_xxh32_update": (None, [_vp, _vp, _sz]),

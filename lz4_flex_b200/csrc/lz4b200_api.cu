@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "lz4b200_frame_batch.cuh"
+#include "lz4b200_frame_encoder.cuh"
 #include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
 #include "lz4b200_solo_kernel.cuh"
@@ -321,6 +322,44 @@ __global__ void frame_tail_kernel(uint8_t *out, FrameHeaderBytes hdr, const uint
         const uint32_t h = fw::xxh32_digest(*content);
         for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
         o += 4;
+    }
+    *written = o;
+}
+
+// ---- streaming frame encoder (lz4b200_frame_encoder) --------------------------------------------------------------------
+// The groups of one call pack back to back after the header; *pos is where the next byte of the call's output goes.
+
+// The header at out[0] when the call opens a frame (hdr.len 0: none), and *pos = hdr.len.
+__global__ void encoder_head_kernel(uint8_t *out, FrameHeaderBytes hdr, uint64_t *pos)
+{
+#pragma unroll
+    for (uint32_t i = 0; i < sizeof hdr.b; i++)
+        if (i < hdr.len) out[i] = hdr.b[i];
+    *pos = hdr.len;
+}
+
+// Moves a group's segment offsets (the scan of its segment sizes, seg_off[0..nb]) to *pos in the call's output, so the
+// gather and the block checksums place it there; the caller then copies seg_off[nb] to *pos.
+__global__ void __launch_bounds__(128) encoder_place_kernel(uint64_t *seg_off, uint32_t nb, const uint64_t *pos)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= nb) seg_off[i] += *pos;
+}
+
+// The end of a call: the EndMark at out[*pos] when the call closes the frame (and the content digest when `content` is
+// given), and the call's length into *written.
+__global__ void encoder_tail_kernel(uint8_t *out, const uint64_t *pos, bool endmark, const lz4b200_xxh32_state *content,
+                                    uint64_t *written)
+{
+    uint64_t o = *pos;
+    if (endmark) {
+        for (int b = 0; b < 4; b++) out[o + b] = 0;
+        o += 4;
+        if (content) {
+            const uint32_t h = fw::xxh32_digest(*content);
+            for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
+            o += 4;
+        }
     }
     *written = o;
 }
@@ -1906,9 +1945,11 @@ namespace {
 // slots, decide compressed-vs-stored per block (frame/compress.rs:301-306) and scan the segment sizes, each of which
 // reserves `trailer` bytes (0, or 4 for a block checksum) after its payload.  *d_total receives the packed size.
 // Everything stays on the device and on `stream`.
+// `host_flags` (one LZ4B200_BLOCK_* per block, host memory) replaces the parse modes the block index gives: the
+// streaming encoder plans them from the stream offset, which a flush shifts off the block grid.
 lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
                                          uint64_t first_block, uint32_t trailer, uint64_t *d_total,
-                                         uint32_t *d_block_sizes, void *stream)
+                                         uint32_t *d_block_sizes, void *stream, const uint8_t *host_flags = nullptr)
 {
     if (!ctx || !block_size || block_size > (8u << 20)) return LZ4B200_INVALID_ARGUMENT;
     const size_t nblocks = (in_len + block_size - 1) / block_size;
@@ -1933,8 +1974,9 @@ lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, 
     make_uniform_desc_kernel<<<(nb + 255) / 256, 256, 0, s>>>(in_len, (uint32_t)block_size, slot, first_block,
                                                              fresh_period(block_size), nb, ctx->d_in_off.p,
                                                              ctx->d_in_len.p, ctx->d_out_off.p, ctx->d_out_cap.p,
-                                                             ctx->d_flags.p);
+                                                             host_flags ? nullptr : ctx->d_flags.p);
     CTX_CUDA(ctx, cudaGetLastError());
+    if (host_flags) CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, host_flags, nb, cudaMemcpyHostToDevice, s));
     BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
                 ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
     lz4b200_status st = launch_compress(ctx, a, (uint32_t)std::min<size_t>(block_size, in_len), s);
@@ -3011,6 +3053,123 @@ lz4b200_status lz4b200_frame_decoder_decode_device(lz4b200_frame_decoder *dec, c
     const lz4b200_status st = decoder_step(dec, s, d_in, n, end_of_input != 0, d_out, out_cap, *step);
     if (st != LZ4B200_CUDA_ERROR) CTX_CUDA(ctx, cudaStreamSynchronize(s));
     return st;
+}
+
+// ---- streaming frame encoder (FrameEncoder over device memory, frame/compress.rs:62-404) -------------------------------
+// The encoder holds what must outlive a call: the stream state of fe::State, the input buffer of one group of whole
+// blocks, the running content hash and the output position of the call.  Descriptors and slots are the context's
+// scratch, so other calls on the context may come between two of its calls.
+struct lz4b200_frame_encoder {
+    lz4b200_ctx *ctx = nullptr;
+    int device = 0;
+    lz4b200_frame_info info{};                // as created; the block size resolves into st
+    fe::State st;
+    uint8_t *d_buf = nullptr;                 // the input buffer: st.group blocks of the open frame's block size
+    size_t buf_bytes = 0;
+    DevBuf<lz4b200_xxh32_state> d_content;    // the running content hash
+    DevBuf<uint64_t> d_pos;                   // the call's output position
+};
+
+lz4b200_status lz4b200_frame_encoder_create(lz4b200_ctx *ctx, const lz4b200_frame_info *info, lz4b200_frame_encoder **out)
+{
+    if (!ctx || !info || !out) return LZ4B200_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (info->linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    const int id = info->block_size_id;
+    if (id != 0 && (id < 4 || id > 7)) return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    lz4b200_frame_encoder *enc = new lz4b200_frame_encoder();
+    enc->ctx = ctx;
+    enc->device = ctx->device;
+    enc->info = *info;
+    enc->st.block_size_id = id;
+    if (!ctx->check(enc->d_content.reserve(1), "encoder content hash") || !ctx->check(enc->d_pos.reserve(1), "encoder position")) {
+        lz4b200_frame_encoder_destroy(enc);
+        return LZ4B200_CUDA_ERROR;
+    }
+    *out = enc;
+    return LZ4B200_OK;
+}
+
+void lz4b200_frame_encoder_destroy(lz4b200_frame_encoder *enc)
+{
+    if (!enc) return;
+    DeviceGuard guard(enc->device);
+    if (enc->d_buf) cudaFree(enc->d_buf);
+    enc->d_content.release(); enc->d_pos.release();
+    delete enc;
+}
+
+size_t lz4b200_frame_encoder_bound(const lz4b200_frame_encoder *enc, size_t n, int op)
+{
+    if (!enc || op < fe::kWrite || op > fe::kFinish) return 0;
+    return fe::call_bound(enc->st, enc->info, enc->ctx->frame_budget, n, op);
+}
+
+uint64_t lz4b200_frame_encoder_content_len(const lz4b200_frame_encoder *enc) { return enc ? enc->st.content_len : 0; }
+
+// One call: plan it on the host (fe::plan_call), then enqueue the header, per step the copy into the buffer and the
+// group's compress, placement, gather, block checksums and content hash, and the tail.  Only kernel arguments and each
+// group's parse modes cross PCIe.
+lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, const uint8_t *d_in, size_t n, int op,
+                                                   uint8_t *d_out, size_t out_cap, uint64_t *d_written, void *stream)
+{
+    if (!enc || !d_written || (!d_out && out_cap)) return LZ4B200_INVALID_ARGUMENT;
+    if (!d_in && n) return LZ4B200_INVALID_ARGUMENT;
+    if (op < fe::kWrite || op > fe::kFinish) return LZ4B200_INVALID_ARGUMENT;
+    lz4b200_ctx *ctx = enc->ctx;
+    if (out_cap < fe::call_bound(enc->st, enc->info, ctx->frame_budget, n, op)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const fe::CallPlan p = fe::plan_call(enc->st, enc->info, ctx->frame_budget, n, op);
+    const size_t bs = fe::block_bytes(p.block_size_id);
+    const size_t want = p.group * bs;
+    if (p.header && want != enc->buf_bytes) {                // the buffer follows the block size and the budget
+        if (enc->d_buf) cudaFree(enc->d_buf);
+        enc->d_buf = nullptr;
+        enc->buf_bytes = 0;
+        CTX_CUDA(ctx, cudaMalloc(reinterpret_cast<void **>(&enc->d_buf), want));
+        enc->buf_bytes = want;
+    }
+
+    lz4b200_frame_info info = enc->info;
+    info.block_size_id = p.block_size_id;
+    FrameHeaderBytes hdr{};
+    if (p.header) hdr.len = (uint8_t)lz4b200_frame_write_header(&info, hdr.b, sizeof hdr.b);
+    uint64_t *pos = enc->d_pos.p;
+    encoder_head_kernel<<<1, 1, 0, s>>>(d_out, hdr, pos);
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (p.header && info.content_checksum) {                 // a new frame's content hash (compress.rs:253)
+        xxh32_reset_kernel<<<1, 1, 0, s>>>(enc->d_content.p, 0);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    for (const fe::Step &st : p.steps) {
+        if (st.len)
+            CTX_CUDA(ctx, cudaMemcpyAsync(enc->d_buf + st.dst, d_in + st.src, st.len, cudaMemcpyDeviceToDevice, s));
+        if (!st.group_len) continue;
+        lz4b200_status r = frame_range_compress_impl(ctx, enc->d_buf, st.group_len, bs, 0, info.block_checksums ? 4u : 0u,
+                                                     nullptr, nullptr, s, p.flags.data() + st.flag0);
+        if (r != LZ4B200_OK) return r;
+        const uint32_t nb = st.nblocks;
+        encoder_place_kernel<<<(nb + 128) / 128, 128, 0, s>>>(ctx->d_seg_off.p, nb, pos);
+        CTX_CUDA(ctx, cudaGetLastError());
+        CTX_CUDA(ctx, cudaMemcpyAsync(pos, ctx->d_seg_off.p + nb, 8, cudaMemcpyDeviceToDevice, s));
+        r = lz4b200_frame_range_pack(ctx, d_out, nullptr, s);
+        if (r != LZ4B200_OK) return r;
+        if (info.block_checksums) {
+            frame_block_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_out, ctx->d_seg_off.p, ctx->d_payload_len.p, nb);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+        if (info.content_checksum) {                          // compress.rs:319-321, in stream order
+            content_hash_kernel<<<1, 256, 0, s>>>(enc->d_content.p, enc->d_buf, st.group_len);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    encoder_tail_kernel<<<1, 1, 0, s>>>(d_out, pos, p.endmark != 0, info.content_checksum ? enc->d_content.p : nullptr,
+                                        d_written);
+    CTX_CUDA(ctx, cudaGetLastError());
+    enc->st = p.next;
+    return (lz4b200_status)p.status;
 }
 
 }  // extern "C"

@@ -448,6 +448,91 @@ class DeviceFrameDecoder:
         return step.consumed, step.written, step.need, bool(step.frame_done), err
 
 
+_ENCODE_WRITE, _ENCODE_FLUSH, _ENCODE_FINISH = 0, 1, 2
+_CONTENT_LENGTH = 109
+
+
+class DeviceFrameEncoder:
+    """FrameEncoder over device memory (lz4b200_frame_encoder): compresses a stream that arrives in device memory in
+    pieces into LZ4 frames in device memory, in device memory that does not grow with the stream (one group of blocks
+    that fits the context's frame budget).  For any sequence of write / flush / finish calls, the concatenated bytes
+    the calls return are what FrameEncoder writes for the same sequence of write_all / flush / try_finish."""
+
+    def __init__(self, frame_info: FrameInfo | None = None, ctx: _block.Context | None = None):
+        self.ctx = ctx or _block.default_context()
+        self._h = None
+        info = frame_info or FrameInfo()
+        if info.block_mode == BlockMode.Linked:
+            raise LinkedBlocksUnsupported()
+        self._info = info
+        ci = info.to_c()
+        h = C.c_void_p()
+        st = _native.lib().lz4b200_frame_encoder_create(self.ctx.handle, C.byref(ci), C.byref(h))
+        if st != 0:
+            raise error_from_status(st, detail=self.ctx.last_cuda_error())
+        self._h = h
+
+    def close(self):
+        if self._h:
+            _native.lib().lz4b200_frame_encoder_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    @staticmethod
+    def _op(flush: bool, finish: bool) -> int:
+        return _ENCODE_FINISH if finish else _ENCODE_FLUSH if flush else _ENCODE_WRITE
+
+    def bound(self, n: int, flush: bool = False, finish: bool = False) -> int:
+        """The most bytes write(n bytes, flush=, finish=) can return in the encoder's current state."""
+        return _native.lib().lz4b200_frame_encoder_bound(self._h, n, self._op(flush, finish))
+
+    def write(self, d_in, out=None, flush: bool = False, finish: bool = False, stream: int | None = None):
+        """write_all(d_in), then flush() or try_finish(); d_in and out are contiguous 1-D torch CUDA uint8 tensors
+        (out None: one of bound() bytes is allocated).  Returns the view of `out` that holds the bytes the call wrote.
+        The work runs on torch's current stream (or `stream`); the call returns once that length has been read back, and
+        d_in may be reused once the stream has passed the call.  A finish that finds a content length other than the
+        FrameInfo's raises ContentLengthError(expected, actual) with the flushed bytes as `.partial`, and closes the
+        frame without an EndMark, as FrameEncoder.try_finish() does."""
+        import torch
+        _device_u8(d_in, "d_in")
+        op = self._op(flush, finish)
+        n = d_in.numel()
+        if out is None:
+            out = torch.empty(self.bound(n, flush, finish), dtype=torch.uint8, device=d_in.device)
+        _device_u8(out, "out")
+        s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+        written = torch.empty(1, dtype=torch.int64, device=out.device)
+        cap = out.numel()
+        st = _native.lib().lz4b200_frame_encoder_encode_device(self._h, d_in.data_ptr() if n else None, n, op,
+                                                               out.data_ptr() if cap else None, cap, written.data_ptr(), s)
+        if st != 0 and st != _CONTENT_LENGTH:
+            raise error_from_status(st, detail=self.ctx.last_cuda_error())
+        if stream is None:
+            w = int(written.item())
+        else:
+            with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=out.device)):
+                w = int(written.item())                                       # copied and synchronised on `stream`
+        if st == _CONTENT_LENGTH:
+            actual = int(_native.lib().lz4b200_frame_encoder_content_len(self._h))
+            raise _with_partial(ContentLengthError(self._info.content_size, actual), out[:w])
+        return out[:w]
+
+    def flush(self, out=None, stream: int | None = None):
+        """flush(): compresses what is buffered; returns the bytes written."""
+        return self.write(self._empty(), out=out, flush=True, stream=stream)
+
+    def finish(self, out=None, stream: int | None = None):
+        """try_finish(): flushes and closes the frame (an empty frame when nothing was written); a later write opens the
+        next frame.  Returns the bytes written."""
+        return self.write(self._empty(), out=out, finish=True, stream=stream)
+
+    def _empty(self):
+        import torch
+        return torch.empty(0, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+
+
 def iter_decompress_device(read_into, out_bytes: int = 8 << 20, in_bytes: int = 16 << 20, ctx: _block.Context | None = None,
                            device=None):
     """Every concatenated frame of a compressed stream that arrives in device memory, decoded in bounded device memory.
