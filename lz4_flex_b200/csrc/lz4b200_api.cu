@@ -143,11 +143,9 @@ __global__ void make_uniform_desc_kernel(uint64_t total_len, uint32_t block, uin
     in_len[i] = (uint32_t)(rem < block ? rem : block);
     out_off[i] = (uint64_t)i * out_stride;
     out_cap[i] = (uint32_t)out_stride;
-    if (flags) {
-        uint64_t k = first_block + i;
-        bool fresh = (k % fresh_period) == 0;
-        flags[i] = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (fresh ? 0u : LZ4B200_BLOCK_CONT));
-    }
+    uint64_t k = first_block + i;
+    bool fresh = (k % fresh_period) == 0;
+    flags[i] = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (fresh ? 0u : LZ4B200_BLOCK_CONT));
 }
 
 // ---- device-resident frame decoder (lz4b200_frame_decompress_next_device) ----------------------------------------------
@@ -283,7 +281,7 @@ __global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *
     content_hash_cta(st, p, n, stage);
 }
 
-// ---- device-resident frame encoder (lz4b200_frame_compress_device) ------------------------------------------------------
+// ---- frame encoders -----------------------------------------------------------------------------------------------------
 
 __global__ void xxh32_reset_kernel(lz4b200_xxh32_state *st, uint32_t seed) { fw::xxh32_reset(*st, seed); }
 
@@ -300,34 +298,14 @@ __global__ void __launch_bounds__(128) frame_block_checksum_kernel(uint8_t *dst,
     for (int b = 0; b < 4; b++) payload[len + b] = (uint8_t)(h >> (8 * b));
 }
 
+// ---- streaming frame encoder (lz4b200_frame_encoder) --------------------------------------------------------------------
+// The groups of one call pack back to back after the header; *pos is where the next byte of the call's output goes.
+
 // The frame header as a kernel argument (FrameInfo::write is at most 15 bytes).
 struct FrameHeaderBytes {
     uint8_t b[19];
     uint8_t len;
 };
-
-// Everything of the frame but its blocks (frame/compress.rs:209-230, header.rs:232-275): the header at out[0], the
-// EndMark after the *seg_total bytes of blocks (null: none), the content digest when `content` is given, and the frame
-// length into *written.
-__global__ void frame_tail_kernel(uint8_t *out, FrameHeaderBytes hdr, const uint64_t *seg_total,
-                                  const lz4b200_xxh32_state *content, uint64_t *written)
-{
-#pragma unroll
-    for (uint32_t i = 0; i < sizeof hdr.b; i++)
-        if (i < hdr.len) out[i] = hdr.b[i];
-    uint64_t o = hdr.len + (seg_total ? *seg_total : 0);
-    for (int b = 0; b < 4; b++) out[o + b] = 0;
-    o += 4;
-    if (content) {
-        const uint32_t h = fw::xxh32_digest(*content);
-        for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
-        o += 4;
-    }
-    *written = o;
-}
-
-// ---- streaming frame encoder (lz4b200_frame_encoder) --------------------------------------------------------------------
-// The groups of one call pack back to back after the header; *pos is where the next byte of the call's output goes.
 
 // The header at out[0] when the call opens a frame (hdr.len 0: none), and *pos = hdr.len.
 __global__ void encoder_head_kernel(uint8_t *out, FrameHeaderBytes hdr, uint64_t *pos)
@@ -336,14 +314,6 @@ __global__ void encoder_head_kernel(uint8_t *out, FrameHeaderBytes hdr, uint64_t
     for (uint32_t i = 0; i < sizeof hdr.b; i++)
         if (i < hdr.len) out[i] = hdr.b[i];
     *pos = hdr.len;
-}
-
-// Moves a group's segment offsets (the scan of its segment sizes, seg_off[0..nb]) to *pos in the call's output, so the
-// gather and the block checksums place it there; the caller then copies seg_off[nb] to *pos.
-__global__ void __launch_bounds__(128) encoder_place_kernel(uint64_t *seg_off, uint32_t nb, const uint64_t *pos)
-{
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i <= nb) seg_off[i] += *pos;
 }
 
 // The end of a call: the EndMark at out[*pos] when the call closes the frame (and the content digest when `content` is
@@ -364,10 +334,13 @@ __global__ void encoder_tail_kernel(uint8_t *out, const uint64_t *pos, bool endm
     *written = o;
 }
 
-// ---- batch frame encoder (lz4b200_frame_compress_batch_device) ----------------------------------------------------------
+// ---- the frame encoders' pipeline (compress_frames) ---------------------------------------------------------------------
 // Many frames per call, their blocks numbered frame after frame (fb::FramePlan, one entry per frame, planned on the host).
 
 static_assert(sizeof(fb::FramePlan) == 64, "one frame's plan is 64 bytes");
+
+// A single frame's plan reaches the device as a kernel argument rather than a copy.
+__global__ void frame_plan_store_kernel(fb::FramePlan *dst, fb::FramePlan p) { *dst = p; }
 
 // The compressor's arguments, one thread per block of the batch (fb::batch_block); dst[b] receives the block's shift
 // into the packed output, to which frame_batch_dst_kernel adds the scan of the segment sizes.
@@ -386,10 +359,15 @@ __global__ void __launch_bounds__(128) frame_batch_blocks_kernel(const fb::Frame
     dst[b] = j.dst_shift;
 }
 
-__global__ void __launch_bounds__(128) frame_batch_dst_kernel(const uint64_t *seg_off, uint32_t nb, uint64_t *dst)
+// With pos_in, the blocks land *pos_in bytes further (a streaming group at its call's position) and thread 0 stores
+// their end to *pos_out, another word than the *pos_in every thread reads.
+__global__ void __launch_bounds__(128) frame_batch_dst_kernel(const uint64_t *seg_off, uint32_t nb, uint64_t *dst,
+                                                              const uint64_t *pos_in, uint64_t *pos_out)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < nb) dst[b] += seg_off[b];
+    const uint64_t pos = pos_in ? *pos_in : 0;
+    if (b < nb) dst[b] += seg_off[b] + pos;
+    if (b == 0 && pos_out) *pos_out = pos + seg_off[nb];
 }
 
 // The content hash of every frame (frame/compress.rs:141,320), one CTA per frame over its input, into states[f].
@@ -643,15 +621,6 @@ int auto_block_size_id(size_t first_write_len)
     if (first_write_len > (256u << 10)) return 7;
     if (first_write_len > (64u << 10)) return 5;
     return 4;
-}
-
-// Number of consecutive full blocks that share one table epoch before FrameEncoder repositions
-// its table (frame/compress.rs:266-271): block k is FRESH iff k % period == 0.
-uint64_t fresh_period(size_t bs)
-{
-    // reposition fires at the first block whose starting offset off satisfies off + bs + 65536 >= 2^31 - 1
-    uint64_t limit = 0x7FFFFFFFull - 65536ull - bs;      // off >= limit
-    return (limit + bs - 1) / bs;
 }
 
 template <typename T> struct DevBuf {
@@ -1941,15 +1910,101 @@ size_t lz4b200_frame_bound(size_t n, const lz4b200_frame_info *info)
 
 namespace {
 
+// Sets what `info` (block size resolved) and the input d_in[in_off, in_off + in_len) decide of the zeroed plan p, the
+// header included; fb::plan_frame places it after the frame before.  p is filled in place, not returned: copying a
+// returned plan into the batch's table stalls the host on every frame.
+void frame_plan(fb::FramePlan &p, const lz4b200_frame_info &info, uint64_t in_off, uint64_t in_len)
+{
+    p.in_off = in_off;
+    p.in_len = in_len;
+    p.bs = (uint32_t)block_size_bytes(info.block_size_id);
+    p.fresh = fb::fresh_period(p.bs);
+    p.hdr_len = (uint8_t)lz4b200_frame_write_header(&info, p.hdr, sizeof p.hdr);
+}
+
+// The pipeline of every frame encoder: enqueues the n >= 1 frames of plan (placed by fb::plan_frame) on `s`.  One plan
+// reaches the device as a kernel argument, more with one copy from pageable memory, which cudaMemcpyAsync stages before
+// it returns, so back-to-back calls never share a host buffer.  Then one thread per block writes the compressor's
+// arguments, one launch compresses every block of every frame, the segment sizes (with room for a checksum after each
+// payload when `block_checksums`) are scanned, one gather packs every [BlockInfo | payload] at its frame's place, and
+// one thread per block writes the block checksums.  max_in_len is launch_compress's bound on the blocks' lengths.  A
+// device position d_pos_in moves every block *d_pos_in bytes further, and *d_pos_out receives the end of the blocks.
+// With `content_checksum` one CTA per frame hashes its content; with d_frame_off one thread per frame writes its
+// header, EndMark, digest (when hashed) and d_frame_off[f], and d_frame_off[n] the total.
+lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::FramePlan *plan, uint32_t n,
+                               uint32_t max_in_len, bool block_checksums, bool content_checksum, uint8_t *d_out,
+                               uint64_t *d_frame_off, const uint64_t *d_pos_in, uint64_t *d_pos_out, cudaStream_t s)
+{
+    const fb::FramePlan &last = plan[n - 1];
+    const uint32_t nb = last.first_block + (uint32_t)fb::frame_blocks(last);
+    CTX_CUDA(ctx, ctx->d_fplan.reserve(n));
+    CTX_CUDA(ctx, ctx->d_slots.reserve(last.slot_base + fb::frame_slot_bytes(last) + 16));
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve((size_t)nb + 1));
+    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb));
+    if (content_checksum) CTX_CUDA(ctx, ctx->d_content.reserve(n));
+    if (n == 1) {
+        frame_plan_store_kernel<<<1, 1, 0, s>>>(ctx->d_fplan.p, plan[0]);
+        CTX_CUDA(ctx, cudaGetLastError());
+    } else {
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_fplan.p, plan, n * sizeof(fb::FramePlan), cudaMemcpyHostToDevice, s));
+    }
+
+    const uint32_t bgrid = (nb + 127) / 128;
+    if (nb) {
+        frame_batch_blocks_kernel<<<bgrid, 128, 0, s>>>(ctx->d_fplan.p, n, nb, ctx->d_in_off.p, ctx->d_in_len.p,
+                                                        ctx->d_out_off.p, ctx->d_out_cap.p, ctx->d_flags.p,
+                                                        ctx->d_gdst.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
+        const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
+        if (st != LZ4B200_OK) return st;
+        frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb,
+                                                                block_checksums ? 4u : 0u, ctx->d_info.p,
+                                                                ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);   // nb == 0: seg_off[0] = 0
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        frame_batch_dst_kernel<<<bgrid, 128, 0, s>>>(ctx->d_seg_off.p, nb, ctx->d_gdst.p, d_pos_in, d_pos_out);
+        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p, ctx->d_payload_len.p,
+                     ctx->d_pick.p, ctx->d_info.p, d_out, ctx->d_gdst.p, nb};
+        gather_segments_kernel<<<std::min<uint32_t>(std::max<uint32_t>(nb, (uint32_t)ctx->sm_count * 2),
+                                                    (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+        CTX_CUDA(ctx, cudaGetLastError());
+        if (block_checksums) {
+            frame_block_checksum_kernel<<<bgrid, 128, 0, s>>>(d_out, ctx->d_gdst.p, ctx->d_payload_len.p, nb);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    if (content_checksum) {
+        frame_batch_content_kernel<<<n, 256, 0, s>>>(d_in, ctx->d_fplan.p, ctx->d_content.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    if (d_frame_off) {
+        frame_batch_tail_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_out, ctx->d_fplan.p, n, ctx->d_seg_off.p,
+                                                                content_checksum ? ctx->d_content.p : nullptr,
+                                                                d_frame_off);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 // Rank-local half of a (possibly sharded) frame, step 1: compress the blocks of [first_block, ...) into the context's
-// slots, decide compressed-vs-stored per block (frame/compress.rs:301-306) and scan the segment sizes, each of which
-// reserves `trailer` bytes (0, or 4 for a block checksum) after its payload.  *d_total receives the packed size.
-// Everything stays on the device and on `stream`.
-// `host_flags` (one LZ4B200_BLOCK_* per block, host memory) replaces the parse modes the block index gives: the
-// streaming encoder plans them from the stream offset, which a flush shifts off the block grid.
-lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
-                                         uint64_t first_block, uint32_t trailer, uint64_t *d_total,
-                                         uint32_t *d_block_sizes, void *stream, const uint8_t *host_flags = nullptr)
+// slots, decide compressed-vs-stored per block (frame/compress.rs:301-306) and scan the segment sizes.  *d_total
+// receives the packed size.  Everything stays on the device and on `stream`.
+lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
+                                            uint64_t first_block, uint64_t *d_total, uint32_t *d_block_sizes, void *stream)
 {
     if (!ctx || !block_size || block_size > (8u << 20)) return LZ4B200_INVALID_ARGUMENT;
     const size_t nblocks = (in_len + block_size - 1) / block_size;
@@ -1972,18 +2027,16 @@ lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, 
     CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(nb + 1));
 
     make_uniform_desc_kernel<<<(nb + 255) / 256, 256, 0, s>>>(in_len, (uint32_t)block_size, slot, first_block,
-                                                             fresh_period(block_size), nb, ctx->d_in_off.p,
+                                                             fb::fresh_period(block_size), nb, ctx->d_in_off.p,
                                                              ctx->d_in_len.p, ctx->d_out_off.p, ctx->d_out_cap.p,
-                                                             host_flags ? nullptr : ctx->d_flags.p);
+                                                             ctx->d_flags.p);
     CTX_CUDA(ctx, cudaGetLastError());
-    if (host_flags) CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, host_flags, nb, cudaMemcpyHostToDevice, s));
     BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
                 ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
     lz4b200_status st = launch_compress(ctx, a, (uint32_t)std::min<size_t>(block_size, in_len), s);
     if (st != LZ4B200_OK) return st;
-    frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb, trailer,
-                                                            ctx->d_info.p, ctx->d_pick.p, ctx->d_seg_size.p,
-                                                            ctx->d_payload_len.p);
+    frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb, 0, ctx->d_info.p,
+                                                            ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
     CTX_CUDA(ctx, cudaGetLastError());
     scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);
     CTX_CUDA(ctx, cudaGetLastError());
@@ -1991,16 +2044,6 @@ lz4b200_status frame_range_compress_impl(lz4b200_ctx *ctx, const uint8_t *d_in, 
     if (d_block_sizes)
         CTX_CUDA(ctx, cudaMemcpyAsync(d_block_sizes, ctx->d_seg_size.p, nb * 4, cudaMemcpyDeviceToDevice, s));
     return LZ4B200_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_in, size_t in_len, size_t block_size,
-                                            uint64_t first_block, uint64_t *d_total, uint32_t *d_block_sizes, void *stream)
-{
-    return frame_range_compress_impl(ctx, d_in, in_len, block_size, first_block, 0, d_total, d_block_sizes, stream);
 }
 
 // Step 2: pack the range's [BlockInfo | payload] segments back to back at d_dst + *d_dst_offset.  d_dst may be PEER
@@ -2074,6 +2117,9 @@ lz4b200_status lz4b200_peer_free(lz4b200_ctx *ctx, void *d_ptr)
     return LZ4B200_OK;
 }
 
+// The blocks are compressed on the device: the input goes over, one plan runs through compress_frames, block checksums
+// included, and the whole frame comes back.  The content digest is computed here over `in` and appended after the
+// EndMark: the host core hashes faster than the device's single serial chain.
 lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const lz4b200_frame_info *info_in,
                                       size_t first_write_len, uint8_t *out, size_t cap, size_t *written)
 {
@@ -2084,54 +2130,31 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
     if (info.block_size_id == 0) info.block_size_id = auto_block_size_id(first_write_len);   // compress.rs:236-238
     if (info.block_size_id < 4 || info.block_size_id > 7) return LZ4B200_INVALID_ARGUMENT;
     if (info.has_content_size && info.content_size != n) return LZ4B200_FRAME_CONTENT_LENGTH; // compress.rs:212-219
-    const size_t bs = block_size_bytes(info.block_size_id);
     if (cap < lz4b200_frame_bound(n, &info)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
     DeviceGuard guard(ctx->device);
     cudaStream_t s = ctx->stream;
 
-    size_t o = lz4b200_frame_write_header(&info, out, cap);
-    const size_t nblocks = (n + bs - 1) / bs;
-    if (nblocks) {
-        const size_t bound = lz4b200_frame_blocks_bound(n, bs);
-        CTX_CUDA(ctx, ctx->d_in.reserve(n + 16));
-        CTX_CUDA(ctx, ctx->d_out.reserve(bound + 16));
-        CTX_CUDA(ctx, ctx->d_off_b.reserve(1));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in, n, cudaMemcpyHostToDevice, s));
-        lz4b200_status st = lz4b200_frame_compress_blocks_device(ctx, ctx->d_in.p, n, bs, 0, ctx->d_out.p, bound,
-                                                                 ctx->d_off_b.p, nullptr, s);
-        if (st != LZ4B200_OK) return st;
-        uint64_t total = 0;
-        CTX_CUDA(ctx, cudaMemcpyAsync(&total, ctx->d_off_b.p, 8, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaStreamSynchronize(s));
-        if (!info.block_checksums) {
-            CTX_CUDA(ctx, cudaMemcpyAsync(out + o, ctx->d_out.p, total, cudaMemcpyDeviceToHost, s));
-            CTX_CUDA(ctx, cudaStreamSynchronize(s));
-            o += total;
-        } else {
-            // block checksum = XXH32 of the payload as written (frame/compress.rs:313-316): host-side walk
-            std::vector<uint8_t> tmp(total);
-            CTX_CUDA(ctx, cudaMemcpyAsync(tmp.data(), ctx->d_out.p, total, cudaMemcpyDeviceToHost, s));
-            CTX_CUDA(ctx, cudaStreamSynchronize(s));
-            size_t p = 0;
-            while (p < total) {
-                uint32_t word = rd32(tmp.data() + p);
-                size_t len = word & 0x7fffffffu;
-                memcpy(out + o, tmp.data() + p, 4 + len);
-                wr32(out + o + 4 + len, lz4b200_xxh32(tmp.data() + p + 4, len, 0));
-                o += 8 + len; p += 4 + len;
-            }
-        }
-    }
-    wr32(out + o, 0); o += 4;                                                            // EndMark: compress.rs:221-223
+    fb::FramePlan plan{};
+    frame_plan(plan, info, 0, n);
+    CTX_CUDA(ctx, ctx->d_in.reserve(n + 16));
+    CTX_CUDA(ctx, ctx->d_out.reserve(lz4b200_frame_bound(n, &info)));
+    CTX_CUDA(ctx, ctx->d_off_b.reserve(2));
+    if (n) CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in, n, cudaMemcpyHostToDevice, s));
+    const lz4b200_status st = compress_frames(ctx, ctx->d_in.p, &plan, 1, (uint32_t)std::min<uint64_t>(n, plan.bs),
+                                              info.block_checksums, false, ctx->d_out.p, ctx->d_off_b.p, nullptr, nullptr, s);
+    if (st != LZ4B200_OK) return st;
+    uint64_t o = 0;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&o, ctx->d_off_b.p + 1, 8, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(out, ctx->d_out.p, o, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
     if (info.content_checksum) { wr32(out + o, lz4b200_xxh32(in, n, 0)); o += 4; }       // compress.rs:224-227
     *written = o;
     return LZ4B200_OK;
 }
 
-// lz4b200_frame_compress for input in device memory, written to device memory without a host synchronisation: the
-// blocks are compressed and packed at d_out + header length with room for their checksums, which one thread per block
-// then writes; the content hash runs over d_in in the context's d_content state; one tail kernel writes the header
-// (a kernel argument), the EndMark, the content digest and *d_written.  Only kernel arguments cross PCIe.
+// lz4b200_frame_compress for input in device memory, written to device memory without a host synchronisation: one plan
+// runs through compress_frames, and the frame's end goes to *d_written.  Only kernel arguments cross PCIe.
 lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
                                              const lz4b200_frame_info *info_in, size_t first_write_len, uint8_t *d_out,
                                              size_t cap, uint64_t *d_written, void *stream)
@@ -2142,50 +2165,23 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
     if (info.block_size_id == 0) info.block_size_id = auto_block_size_id(first_write_len);   // compress.rs:236-238
     if (info.block_size_id < 4 || info.block_size_id > 7) return LZ4B200_INVALID_ARGUMENT;
     if (info.has_content_size && info.content_size != n) return LZ4B200_FRAME_CONTENT_LENGTH; // compress.rs:212-219
-    const size_t bs = block_size_bytes(info.block_size_id);
     if (cap < lz4b200_frame_bound(n, &info)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
     DeviceGuard guard(ctx->device);
     cudaStream_t s = (cudaStream_t)stream;
 
-    FrameHeaderBytes hdr{};
-    hdr.len = (uint8_t)lz4b200_frame_write_header(&info, hdr.b, sizeof hdr.b);
-    const uint64_t *seg_total = nullptr;
-    if (n) {
-        lz4b200_status st = frame_range_compress_impl(ctx, d_in, n, bs, 0, info.block_checksums ? 4u : 0u, nullptr,
-                                                      nullptr, s);
-        if (st != LZ4B200_OK) return st;
-        st = lz4b200_frame_range_pack(ctx, d_out + hdr.len, nullptr, s);
-        if (st != LZ4B200_OK) return st;
-        const uint32_t nb = ctx->range_nb;
-        if (info.block_checksums) {
-            frame_block_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_out + hdr.len, ctx->d_seg_off.p,
-                                                                         ctx->d_payload_len.p, nb);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
-        seg_total = ctx->d_seg_off.p + nb;
-    }
-    const lz4b200_xxh32_state *content = nullptr;
-    if (info.content_checksum) {                                                         // compress.rs:141,320
-        CTX_CUDA(ctx, ctx->d_content.reserve(1));
-        xxh32_reset_kernel<<<1, 1, 0, s>>>(ctx->d_content.p, 0);
-        CTX_CUDA(ctx, cudaGetLastError());
-        if (n) {
-            content_hash_kernel<<<1, 256, 0, s>>>(ctx->d_content.p, d_in, n);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
-        content = ctx->d_content.p;
-    }
-    frame_tail_kernel<<<1, 1, 0, s>>>(d_out, hdr, seg_total, content, d_written);
-    CTX_CUDA(ctx, cudaGetLastError());
+    fb::FramePlan plan{};
+    frame_plan(plan, info, 0, n);
+    CTX_CUDA(ctx, ctx->d_off_b.reserve(2));
+    const lz4b200_status st = compress_frames(ctx, d_in, &plan, 1, (uint32_t)std::min<uint64_t>(n, plan.bs),
+                                              info.block_checksums, info.content_checksum, d_out, ctx->d_off_b.p,
+                                              nullptr, nullptr, s);
+    if (st != LZ4B200_OK) return st;
+    CTX_CUDA(ctx, cudaMemcpyAsync(d_written, ctx->d_off_b.p + 1, 8, cudaMemcpyDeviceToDevice, s));
     return LZ4B200_OK;
 }
 
-// lz4b200_frame_compress_device for each of many inputs, frames packed back to back, in one call.  The host plans every
-// frame (fb::plan_frame) and uploads the plan with one copy from pageable memory, which cudaMemcpyAsync stages before it
-// returns, so back-to-back calls never share a host buffer.  Then, all on `stream`: one thread per block writes the
-// compressor's arguments, one launch compresses every block of every frame, the segment sizes are scanned, one gather
-// packs every [BlockInfo | payload] at its frame's place, one thread per block writes the block checksums, one CTA per
-// frame hashes its content, and one thread per frame writes its header, EndMark, digest and offset.
+// lz4b200_frame_compress_device for each of many inputs, frames packed back to back, in one call: the host plans every
+// frame (fb::plan_frame) and compress_frames enqueues them all on `stream`.
 lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *in_off,
                                                    const uint64_t *in_len, const lz4b200_frame_info *info,
                                                    uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
@@ -2200,24 +2196,19 @@ lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8
     if ((id != 0 && (id < 4 || id > 7)) || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
     const uint32_t tail = info->content_checksum ? 8u : 4u;
     std::vector<fb::FramePlan> plan(nframes);
-    uint64_t nblocks = 0, bound = 0, slots = 0, max_len = 0;
+    uint64_t nblocks = 0, bound = 0, max_len = 0;
     bool small = false;                                     // some block has at most 64 KiB
     for (size_t f = 0; f < nframes; f++) {
         lz4b200_frame_info fi = *info;
         if (id == 0) fi.block_size_id = auto_block_size_id(in_len[f]);                      // compress.rs:236-238
         fi.content_size = in_len[f];
         fb::FramePlan &p = plan[f];
-        p.in_off = in_off[f];
-        p.in_len = in_len[f];
-        p.bs = (uint32_t)block_size_bytes(fi.block_size_id);
-        p.fresh = (uint32_t)fresh_period(p.bs);
-        p.hdr_len = (uint8_t)lz4b200_frame_write_header(&fi, p.hdr, sizeof p.hdr);
+        frame_plan(p, fi, in_off[f], in_len[f]);
         const uint64_t nb = fb::frame_blocks(p);
         if (nblocks + nb > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
         fb::plan_frame(p, f ? &plan[f - 1] : nullptr, tail);
         nblocks += nb;
         bound += lz4b200_frame_bound(p.in_len, &fi);
-        slots += fb::frame_slot_bytes(p);
         if (nb) {
             max_len = std::max<uint64_t>(max_len, std::min<uint64_t>(p.in_len, p.bs));
             small = small || p.in_len - (nb - 1) * p.bs <= 65536u;               // the last block is the shortest
@@ -2230,60 +2221,11 @@ lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8
         CTX_CUDA(ctx, cudaMemsetAsync(d_frame_off, 0, 8, s));
         return LZ4B200_OK;
     }
-    const uint32_t n = (uint32_t)nframes, nb = (uint32_t)nblocks;
-    CTX_CUDA(ctx, ctx->d_fplan.reserve(n));
-    CTX_CUDA(ctx, ctx->d_slots.reserve(slots + 16));
-    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve((size_t)nb + 1));
-    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb));
-    if (info->content_checksum) CTX_CUDA(ctx, ctx->d_content.reserve(n));
-    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_fplan.p, plan.data(), n * sizeof(fb::FramePlan), cudaMemcpyHostToDevice, s));
-
-    const uint32_t bgrid = (nb + 127) / 128;
-    if (nb) {
-        frame_batch_blocks_kernel<<<bgrid, 128, 0, s>>>(ctx->d_fplan.p, n, nb, ctx->d_in_off.p, ctx->d_in_len.p,
-                                                        ctx->d_out_off.p, ctx->d_out_cap.p, ctx->d_flags.p,
-                                                        ctx->d_gdst.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-        // blocks on both sides of 64 KiB run both encoders whatever the bound says; an unknown bound (0) makes the
-        // launcher's record name both
-        const uint32_t max_in_len = small && max_len > 65536u ? 0u : (uint32_t)max_len;
-        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
-                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
-        const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
-        if (st != LZ4B200_OK) return st;
-        frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb,
-                                                                info->block_checksums ? 4u : 0u, ctx->d_info.p,
-                                                                ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-    }
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);   // nb == 0: seg_off[0] = 0
-    CTX_CUDA(ctx, cudaGetLastError());
-    if (nb) {
-        frame_batch_dst_kernel<<<bgrid, 128, 0, s>>>(ctx->d_seg_off.p, nb, ctx->d_gdst.p);
-        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p, ctx->d_payload_len.p,
-                     ctx->d_pick.p, ctx->d_info.p, d_out, ctx->d_gdst.p, nb};
-        gather_segments_kernel<<<std::min<uint32_t>(std::max<uint32_t>(nb, (uint32_t)ctx->sm_count * 2),
-                                                    (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
-        CTX_CUDA(ctx, cudaGetLastError());
-        if (info->block_checksums) {
-            frame_block_checksum_kernel<<<bgrid, 128, 0, s>>>(d_out, ctx->d_gdst.p, ctx->d_payload_len.p, nb);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
-    }
-    if (info->content_checksum) {
-        frame_batch_content_kernel<<<n, 256, 0, s>>>(d_in, ctx->d_fplan.p, ctx->d_content.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-    }
-    frame_batch_tail_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_out, ctx->d_fplan.p, n, ctx->d_seg_off.p,
-                                                            info->content_checksum ? ctx->d_content.p : nullptr,
-                                                            d_frame_off);
-    CTX_CUDA(ctx, cudaGetLastError());
-    return LZ4B200_OK;
+    // blocks on both sides of 64 KiB run both encoders whatever the bound says; an unknown bound (0) makes the
+    // launcher's record name both
+    const uint32_t max_in_len = small && max_len > 65536u ? 0u : (uint32_t)max_len;
+    return compress_frames(ctx, d_in, plan.data(), (uint32_t)nframes, max_in_len, info->block_checksums,
+                           info->content_checksum, d_out, d_frame_off, nullptr, nullptr, s);
 }
 
 namespace {
@@ -3067,7 +3009,8 @@ struct lz4b200_frame_encoder {
     uint8_t *d_buf = nullptr;                 // the input buffer: st.group blocks of the open frame's block size
     size_t buf_bytes = 0;
     DevBuf<lz4b200_xxh32_state> d_content;    // the running content hash
-    DevBuf<uint64_t> d_pos;                   // the call's output position
+    DevBuf<uint64_t> d_pos;                   // the call's output position, double-buffered: group g moves it from
+                                              // d_pos[g % 2] to d_pos[(g + 1) % 2]
 };
 
 lz4b200_status lz4b200_frame_encoder_create(lz4b200_ctx *ctx, const lz4b200_frame_info *info, lz4b200_frame_encoder **out)
@@ -3083,7 +3026,7 @@ lz4b200_status lz4b200_frame_encoder_create(lz4b200_ctx *ctx, const lz4b200_fram
     enc->device = ctx->device;
     enc->info = *info;
     enc->st.block_size_id = id;
-    if (!ctx->check(enc->d_content.reserve(1), "encoder content hash") || !ctx->check(enc->d_pos.reserve(1), "encoder position")) {
+    if (!ctx->check(enc->d_content.reserve(1), "encoder content hash") || !ctx->check(enc->d_pos.reserve(2), "encoder position")) {
         lz4b200_frame_encoder_destroy(enc);
         return LZ4B200_CUDA_ERROR;
     }
@@ -3108,9 +3051,9 @@ size_t lz4b200_frame_encoder_bound(const lz4b200_frame_encoder *enc, size_t n, i
 
 uint64_t lz4b200_frame_encoder_content_len(const lz4b200_frame_encoder *enc) { return enc ? enc->st.content_len : 0; }
 
-// One call: plan it on the host (fe::plan_call), then enqueue the header, per step the copy into the buffer and the
-// group's compress, placement, gather, block checksums and content hash, and the tail.  Only kernel arguments and each
-// group's parse modes cross PCIe.
+// One call: plan it on the host (fe::plan_call), then enqueue the header, per step the copy into the buffer, the
+// group's plan through compress_frames at the call's position and its content hash, and the tail.  Only kernel
+// arguments cross PCIe.
 lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, const uint8_t *d_in, size_t n, int op,
                                                    uint8_t *d_out, size_t out_cap, uint64_t *d_written, void *stream)
 {
@@ -3143,29 +3086,23 @@ lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, c
         xxh32_reset_kernel<<<1, 1, 0, s>>>(enc->d_content.p, 0);
         CTX_CUDA(ctx, cudaGetLastError());
     }
+    uint32_t g = 0;                                          // groups so far: the position is at pos[g % 2]
     for (const fe::Step &st : p.steps) {
         if (st.len)
             CTX_CUDA(ctx, cudaMemcpyAsync(enc->d_buf + st.dst, d_in + st.src, st.len, cudaMemcpyDeviceToDevice, s));
         if (!st.group_len) continue;
-        lz4b200_status r = frame_range_compress_impl(ctx, enc->d_buf, st.group_len, bs, 0, info.block_checksums ? 4u : 0u,
-                                                     nullptr, nullptr, s, p.flags.data() + st.flag0);
+        const fb::FramePlan plan = fe::group_plan(st, bs);
+        const lz4b200_status r = compress_frames(ctx, enc->d_buf, &plan, 1,
+                                                 (uint32_t)std::min<uint64_t>(st.group_len, bs), info.block_checksums,
+                                                 false, d_out, nullptr, pos + g % 2, pos + (g + 1) % 2, s);
         if (r != LZ4B200_OK) return r;
-        const uint32_t nb = st.nblocks;
-        encoder_place_kernel<<<(nb + 128) / 128, 128, 0, s>>>(ctx->d_seg_off.p, nb, pos);
-        CTX_CUDA(ctx, cudaGetLastError());
-        CTX_CUDA(ctx, cudaMemcpyAsync(pos, ctx->d_seg_off.p + nb, 8, cudaMemcpyDeviceToDevice, s));
-        r = lz4b200_frame_range_pack(ctx, d_out, nullptr, s);
-        if (r != LZ4B200_OK) return r;
-        if (info.block_checksums) {
-            frame_block_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_out, ctx->d_seg_off.p, ctx->d_payload_len.p, nb);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
+        g++;
         if (info.content_checksum) {                          // compress.rs:319-321, in stream order
             content_hash_kernel<<<1, 256, 0, s>>>(enc->d_content.p, enc->d_buf, st.group_len);
             CTX_CUDA(ctx, cudaGetLastError());
         }
     }
-    encoder_tail_kernel<<<1, 1, 0, s>>>(d_out, pos, p.endmark != 0, info.content_checksum ? enc->d_content.p : nullptr,
+    encoder_tail_kernel<<<1, 1, 0, s>>>(d_out, pos + g % 2, p.endmark != 0, info.content_checksum ? enc->d_content.p : nullptr,
                                         d_written);
     CTX_CUDA(ctx, cudaGetLastError());
     enc->st = p.next;

@@ -1,12 +1,12 @@
-// lz4b200_frame_batch.cuh — the plan of the batch frame encoder (lz4b200_frame_compress_batch_device), shared by the
-// host and the device.
+// lz4b200_frame_batch.cuh — the plan every frame encoder runs (lz4b200_frame_compress, _compress_device,
+// _compress_batch_device and the streaming encoder's groups), shared by the host and the device.
 //
-// The host plans every frame of a batch in one pass (plan_frame) and uploads the table.  The blocks of all frames are
-// numbered frame after frame and compressed in one launch; one GPU thread per block finds its frame by binary search
-// over the frames' first block indices and derives its input range, its scratch slot, its parse mode and where its
-// [BlockInfo | payload (| checksum)] segment lands in the packed output (batch_block).  Frames lie back to back: frame
-// f starts at seg_off[first_block] + ovh, where seg_off is the exclusive scan of every block's segment size and ovh the
-// header, EndMark and digest bytes of the frames before it (frame_place).
+// The host plans every frame of a batch in one pass (plan_frame) and hands the table to the device.  The blocks of all
+// frames are numbered frame after frame and compressed in one launch; one GPU thread per block finds its frame by
+// binary search over the frames' first block indices and derives its input range, its scratch slot, its parse mode and
+// where its [BlockInfo | payload (| checksum)] segment lands in the packed output (batch_block).  Frames lie back to
+// back: frame f starts at seg_off[first_block] + ovh, where seg_off is the exclusive scan of every block's segment size
+// and ovh the header, EndMark and digest bytes of the frames before it (frame_place).
 // The header also compiles for the host alone (tests/cpp/frame_batch_host.cpp) for the CPU tests.
 #pragma once
 #include "lz4b200_frame_walk.cuh"
@@ -21,14 +21,23 @@ struct FramePlan {
     uint64_t ovh;                  // header, EndMark and digest bytes of the frames before
     uint32_t first_block;          // batch index of the frame's block 0
     uint32_t bs;                   // the frame's block size
-    uint32_t fresh;                // table epoch: block k of the frame is FRESH iff k % fresh == 0 (frame/compress.rs:266-271)
+    uint32_t fresh;                // table epoch (frame/compress.rs:266-271): block k of the frame is FRESH iff
+                                   // k >= first_fresh and (k - first_fresh) % fresh == 0
     uint8_t hdr[15];               // FrameInfo::write (header.rs:232-275): at most 15 bytes without a dictionary id
     uint8_t hdr_len;
-    uint32_t pad;
+    uint32_t first_fresh;          // 0 for a whole frame; after a flush a streaming group's epochs are off its block grid
 };
 
 // The scratch slot of a block of `len` input bytes: lz4b200_max_output_size(len) rounded up to 16 bytes.
 FW_FN uint64_t slot_bytes_for(uint64_t len) { return (20ull + len * 110ull / 100ull + 15ull) & ~15ull; }
+
+// Full blocks of bs bytes that share one table epoch: FrameEncoder repositions its table at the first block whose
+// stream offset off has off + bs + 64 KiB >= 2^31 - 1 (frame/compress.rs:266-271).
+FW_FN uint32_t fresh_period(uint64_t bs)
+{
+    const uint64_t limit = 0x7FFFFFFFull - 65536ull - bs;
+    return (uint32_t)((limit + bs - 1) / bs);
+}
 
 FW_FN uint64_t frame_blocks(const FramePlan &p) { return (p.in_len + p.bs - 1) / p.bs; }
 
@@ -84,7 +93,8 @@ FW_FN BlockJob batch_block(const FramePlan *p, uint32_t nframes, uint32_t b)
     j.out_off = q.slot_base + (uint64_t)j.k * slot_bytes_for(q.bs);
     j.out_cap = (uint32_t)slot_bytes_for(j.in_len);
     j.dst_shift = q.ovh + q.hdr_len;
-    j.flags = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (j.k % q.fresh == 0 ? 0u : LZ4B200_BLOCK_CONT));
+    const bool fresh = j.k >= q.first_fresh && (j.k - q.first_fresh) % q.fresh == 0;
+    j.flags = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (fresh ? 0u : LZ4B200_BLOCK_CONT));
     return j;
 }
 

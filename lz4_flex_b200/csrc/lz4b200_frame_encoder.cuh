@@ -51,11 +51,11 @@ struct State {
 };
 
 // One step of a call: copy d_in[src, src + len) to buffer[dst, dst + len) (len may be 0), then, when group_len > 0,
-// compress buffer[0, group_len) as nblocks blocks whose parse modes are flags[flag0, flag0 + nblocks).
+// compress buffer[0, group_len) as nblocks blocks, of which block first_fresh is the first FRESH one (group_plan).
 struct Step {
     uint64_t src, dst, len;
     uint64_t group_len;
-    uint32_t nblocks, flag0;
+    uint32_t nblocks, first_fresh;
 };
 
 // A call, planned: the header first when the call opens a frame, then the steps, then the EndMark (and the content
@@ -68,10 +68,21 @@ struct CallPlan {
     int32_t block_size_id = 0;    // the frame's block size (resolved)
     uint64_t group = 0;           // blocks per group
     std::vector<Step> steps;
-    std::vector<uint8_t> flags;   // LZ4B200_BLOCK_* of every block the call cuts, in order
     std::vector<uint64_t> block_off;   // src_stream_offset each block is compressed at (after the reposition check)
     State next;
 };
+
+// The frame plan of a compressing step: its group's blocks with neither header nor tail.  Only the last block of a
+// group can be short, so after the first FRESH block the table repositions every fb::fresh_period blocks.
+static inline fb::FramePlan group_plan(const Step &st, uint64_t bs)
+{
+    fb::FramePlan p{};
+    p.in_len = st.group_len;
+    p.bs = (uint32_t)bs;
+    p.fresh = fb::fresh_period(bs);
+    p.first_fresh = st.first_fresh;
+    return p;
+}
 
 // begin_frame (compress.rs:234-258): resolve Auto from the length of the write that opens the frame, and reset the
 // stream state when the frame before had content.  The buffer is empty whenever no frame is open.
@@ -87,15 +98,16 @@ static inline void begin_frame(State &s, uint64_t len, uint64_t budget)
 }
 
 // write_block (compress.rs:261-371) for the blocks of buffer[0, len): each block's parse mode follows the stream offset
-// after the reposition check, FRESH exactly when it is 0.
+// after the reposition check, FRESH exactly when it is 0.  A group without a FRESH block gets first_fresh = nblocks.
 static inline void cut_blocks(State &s, CallPlan &p, uint64_t len)
 {
     const uint64_t bs = block_bytes(s.block_size_id);
-    Step st{0, 0, 0, len, (uint32_t)((len + bs - 1) / bs), (uint32_t)p.flags.size()};
-    for (uint64_t o = 0; o < len; o += bs) {
-        const uint64_t n = len - o < bs ? len - o : bs;
+    const uint32_t nblocks = (uint32_t)((len + bs - 1) / bs);
+    Step st{0, 0, 0, len, nblocks, nblocks};
+    for (uint32_t k = 0; k < nblocks; k++) {
+        const uint64_t n = len - k * bs < bs ? len - k * bs : bs;
         if (s.stream_offset + bs + kWindow >= kRepositionLimit) s.stream_offset = 0;   // compress.rs:267-271
-        p.flags.push_back((uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (s.stream_offset ? LZ4B200_BLOCK_CONT : 0u)));
+        if (s.stream_offset == 0 && st.first_fresh == nblocks) st.first_fresh = k;
         p.block_off.push_back(s.stream_offset);
         s.stream_offset += n;                                                         // compress.rs:366
     }
@@ -103,7 +115,7 @@ static inline void cut_blocks(State &s, CallPlan &p, uint64_t len)
     if (!p.steps.empty() && p.steps.back().group_len == 0) {   // the copy that filled the buffer compresses it
         p.steps.back().group_len = st.group_len;
         p.steps.back().nblocks = st.nblocks;
-        p.steps.back().flag0 = st.flag0;
+        p.steps.back().first_fresh = st.first_fresh;
     } else {
         p.steps.push_back(st);
     }

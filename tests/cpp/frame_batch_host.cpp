@@ -3,7 +3,8 @@
 // UndefinedBehaviorSanitizer and driven by tests/test_frame_batch_host.py.  Test infrastructure only: nothing in the
 // product links or runs this.
 //
-// stdin: records of  u32 nframes | u32 tail_len | nframes x (u64 in_off | u64 in_len | u32 bs | u32 fresh | u8 hdr_len)
+// stdin: records of  u32 nframes | u32 tail_len |
+//                    nframes x (u64 in_off | u64 in_len | u32 bs | u32 fresh | u32 first_fresh | u8 hdr_len)
 //        followed by one u32 segment size per block of the batch.
 // Each record prints "nblocks slots", then per block "frame k in_off in_len out_off out_cap flags dst" (dst: the
 // segment's offset in the packed output), then per frame "start endmark".
@@ -28,7 +29,7 @@ int main()
         for (uint32_t f = 0; f < n; f++) {
             FramePlan &p = plan[f];
             if (!read_exact(&p.in_off, 8) || !read_exact(&p.in_len, 8) || !read_exact(&p.bs, 4) ||
-                !read_exact(&p.fresh, 4) || !read_exact(&p.hdr_len, 1))
+                !read_exact(&p.fresh, 4) || !read_exact(&p.first_fresh, 4) || !read_exact(&p.hdr_len, 1))
                 return 2;
             plan_frame(p, f ? &plan[f - 1] : nullptr, tail);
             nb += frame_blocks(p);

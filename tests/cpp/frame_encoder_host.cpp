@@ -6,7 +6,8 @@
 // stdin: records of  u32 nops | i32 block_size_id | u8 block_checksums | u8 content_checksum | u8 has_content_size |
 //                    u64 content_size | u64 budget, then nops x (u64 n | u8 op).
 // Each call prints "status header endmark block_size_id group bound nsteps nblocks buffered content_len" (the last two
-// after the call), then per step "src dst len group_len nblocks flag0", then per block "flags stream_offset".
+// after the call), then per step "src dst len group_len nblocks b0" (b0: the call's blocks before the step's group), then
+// per block "flags stream_offset", the flags being what fb::batch_block gives the block in its step's group_plan.
 #include <cstdint>
 #include <cstdio>
 #include <vector>
@@ -41,12 +42,18 @@ int main()
             const CallPlan p = plan_call(s, info, budget, n, op);
             printf("%d %u %u %d %llu %llu %zu %zu %llu %llu\n", p.status, (unsigned)p.header, (unsigned)p.endmark,
                    p.block_size_id, (unsigned long long)p.group, (unsigned long long)bound, p.steps.size(),
-                   p.flags.size(), (unsigned long long)p.next.buffered, (unsigned long long)p.next.content_len);
-            for (const Step &st : p.steps)
-                printf("%llu %llu %llu %llu %u %u\n", (unsigned long long)st.src, (unsigned long long)st.dst,
-                       (unsigned long long)st.len, (unsigned long long)st.group_len, st.nblocks, st.flag0);
-            for (size_t b = 0; b < p.flags.size(); b++)
-                printf("%u %llu\n", (unsigned)p.flags[b], (unsigned long long)p.block_off[b]);
+                   p.block_off.size(), (unsigned long long)p.next.buffered, (unsigned long long)p.next.content_len);
+            std::vector<uint8_t> flags;
+            for (const Step &st : p.steps) {
+                printf("%llu %llu %llu %llu %u %zu\n", (unsigned long long)st.src, (unsigned long long)st.dst,
+                       (unsigned long long)st.len, (unsigned long long)st.group_len, st.nblocks, flags.size());
+                if (!st.group_len) continue;
+                const lz4b200::fb::FramePlan g = group_plan(st, block_bytes(p.block_size_id));
+                for (uint32_t k = 0; k < st.nblocks; k++) flags.push_back(lz4b200::fb::batch_block(&g, 1, k).flags);
+            }
+            if (flags.size() != p.block_off.size()) return 3;
+            for (size_t b = 0; b < flags.size(); b++)
+                printf("%u %llu\n", (unsigned)flags[b], (unsigned long long)p.block_off[b]);
             s = p.next;
         }
     }

@@ -28,8 +28,8 @@ from frame_device_probe import card, timed  # noqa: E402
 from lz4_flex_b200 import _native, block, corpus, frame  # noqa: E402
 from lz4_flex_b200.frame import BlockSize, FrameInfo  # noqa: E402
 
-KERNELS = ("lz4_compress_blocks", "frame_block_checksum_kernel", "content_hash_kernel", "gather_segments_kernel",
-           "frame_tail_kernel")
+KERNELS = ("lz4_compress_blocks", "frame_block_checksum_kernel", "frame_batch_content_kernel", "gather_segments_kernel",
+           "frame_batch_tail_kernel")
 
 
 def kernel_times(fn, trace_path=None):
@@ -109,7 +109,7 @@ def main():
         for _ in range(2):
             t["device"].append(timed(dev)); t["floor"].append(timed(floor)); t["host"].append(timed(host))
         k, _ = kernel_times(dev)
-        hash_ms = k["content_hash_kernel"][1]
+        hash_ms = k["frame_batch_content_kernel"][1]
         row = {"frame": name, "input_bytes": int(n), "frame_bytes": hw.value, "blocks": (n + bsz - 1) // bsz,
                "ms": {m: [round(v, 2) for v in vs] for m, vs in t.items()},
                "kernels_ms": {m: {"launches": c, "ms": round(ms, 3)} for m, (c, ms) in k.items()},

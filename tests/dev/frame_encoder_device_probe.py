@@ -11,7 +11,8 @@ Prints the card and its power limit, then for
 the time of each (one checked warm-up, then two passes alternating with the one-shot call; host clock around a
 sequence of calls that ends in a device synchronise; the calls themselves do not synchronise), the context's device
 bytes after the run and the encoder's buffer.  With --profile, one extra pass of a few runs under torch.profiler gives
-the summed CUDA time per kernel (buffer copy, compress, gather, block checksum, content hash)."""
+the summed CUDA time per kernel (buffer copy, plan, compress, scan and placement, gather, block checksum, content
+hash)."""
 import argparse
 import ctypes as C
 import json

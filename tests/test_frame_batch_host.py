@@ -1,7 +1,7 @@
 """CPU tests of the batch frame encoder's plan (lz4_flex_b200/csrc/lz4b200_frame_batch.cuh), compiled for the host by
 g++ under AddressSanitizer and UndefinedBehaviorSanitizer (tests/cpp/frame_batch_host.cpp): on random lists of frame
-lengths and block sizes, every block's frame, frame-local index, input range, scratch slot, FRESH/CONT mode and packed
-destination, and every frame's place in the packed output, against a Python restatement.  No GPU needed."""
+lengths, block sizes and first FRESH blocks, every block's frame, frame-local index, input range, scratch slot, FRESH/CONT
+mode and packed destination, and every frame's place in the packed output, against a Python restatement.  No GPU needed."""
 import os
 import shutil
 import struct
@@ -42,7 +42,8 @@ def planner():
 
 def fresh_period(bs):
     """FrameEncoder repositions its table at the first block whose offset off has off + bs + 64 KiB >= 2^31 - 1
-    (frame/compress.rs:266-271); block k of a frame is FRESH iff k is a multiple of the period."""
+    (frame/compress.rs:266-271); block k of a frame is FRESH iff k >= first_fresh and k - first_fresh is a multiple of
+    the period."""
     limit = 0x7FFFFFFF - 65536 - bs
     return -(-limit // bs)
 
@@ -52,16 +53,17 @@ def slot(n):
 
 
 def py_plan(frames, tail, seg):
-    """frames: [(in_off, in_len, bs, hdr_len)]; seg: every block's segment size.  Returns (blocks, places)."""
+    """frames: [(in_off, in_len, bs, hdr_len, first_fresh)]; seg: every block's segment size.  Returns (blocks,
+    places)."""
     blocks, places = [], []
     seg_off = np.concatenate([[0], np.cumsum(np.asarray(seg, dtype=np.int64))]).tolist()
     b, slot_base, ovh = 0, 0, 0
-    for f, (in_off, n, bs, hdr_len) in enumerate(frames):
+    for f, (in_off, n, bs, hdr_len, ff) in enumerate(frames):
         nb = -(-n // bs)
         first = b
         for k in range(nb):
             ln = min(bs, n - k * bs)
-            flags = HASH5_ALWAYS | (0 if k % fresh_period(bs) == 0 else CONT)
+            flags = HASH5_ALWAYS | (0 if k >= ff and (k - ff) % fresh_period(bs) == 0 else CONT)
             blocks.append((f, k, in_off + k * bs, ln, slot_base, slot(ln), flags, seg_off[b] + ovh + hdr_len))
             slot_base += slot(ln)
             b += 1
@@ -72,7 +74,7 @@ def py_plan(frames, tail, seg):
 
 def record(frames, tail, seg):
     head = struct.pack("<II", len(frames), tail)
-    body = b"".join(struct.pack("<QQIIB", o, n, bs, fresh_period(bs), h) for o, n, bs, h in frames)
+    body = b"".join(struct.pack("<QQIIIB", o, n, bs, fresh_period(bs), ff, h) for o, n, bs, h, ff in frames)
     return head + body + np.asarray(seg, dtype=np.uint32).tobytes()
 
 
@@ -90,7 +92,8 @@ def random_batch(rng):
             n = int(rng.integers(0, 5 * bs + 2))
             if rng.random() < 0.3:
                 n = bs * int(rng.integers(0, 4))           # a whole number of blocks
-        frames.append((off, n, bs, int(rng.choice([7, 15]))))
+        ff = 0 if rng.random() < 0.5 else int(rng.integers(0, 6))   # a streaming group's blocks after a flush
+        frames.append((off, n, bs, int(rng.choice([7, 15])), ff))
         off += n + int(rng.integers(0, 17))
     return frames
 
@@ -100,7 +103,7 @@ def test_plan_matches_restatement(planner):
     cases = []
     for _ in range(1500):
         frames = random_batch(rng)
-        nb = sum(-(-n // bs) for _, n, bs, _ in frames)
+        nb = sum(-(-n // bs) for _, n, bs, _, _ in frames)
         seg = rng.integers(8, 1 << 20, size=nb).tolist()
         cases.append((frames, int(rng.choice([4, 8])), seg))
     out = planner(b"".join(record(*c) for c in cases))
@@ -117,7 +120,8 @@ def test_plan_matches_restatement(planner):
         # packed: every frame starts where the one before it ends
         for f in range(1, len(frames)):
             assert got_places[f][0] == got_places[f - 1][1] + tail
-        nonfresh_after_first += sum(1 for blk in got_blocks if blk[1] and blk[0] and not blk[6] & CONT)
+        nonfresh_after_first += sum(1 for blk in got_blocks
+                                    if blk[1] != frames[blk[0]][4] and blk[0] and not blk[6] & CONT)
     assert pos == len(out)
     assert nonfresh_after_first == 0
 
@@ -129,10 +133,12 @@ def test_slot_is_max_output_size():
 
 
 def test_fresh_is_frame_local(planner):
-    """A 513-block frame of 4 MiB blocks after frames with blocks: its block 511 is FRESH by its frame-local index."""
+    """A 513-block frame of 4 MiB blocks after frames with blocks: its block 511 is FRESH by its frame-local index.  A
+    frame whose first FRESH block is 1 (a streaming group after a flush) repositions at its block 512."""
     bs = 4 << 20
-    frames = [(0, 3 * 65536 + 5, 64 << 10, 7), (3 * 65536 + 5, 10, bs, 15), (3 * 65536 + 15, 513 * bs, bs, 15)]
-    nb = 4 + 1 + 513
+    frames = [(0, 3 * 65536 + 5, 64 << 10, 7, 0), (3 * 65536 + 5, 10, bs, 15, 0), (3 * 65536 + 15, 513 * bs, bs, 15, 0),
+              (0, 513 * bs, bs, 0, 1)]
+    nb = 4 + 1 + 513 + 513
     seg = [100] * nb
     out = planner(record(frames, 8, seg))
     blocks = out[1:1 + nb]
@@ -140,5 +146,6 @@ def test_fresh_is_frame_local(planner):
     assert len(big) == 513
     fresh = [blk[1] for blk in big if not blk[6] & CONT]
     assert fresh == [0, 511]
+    assert [blk[1] for blk in blocks if blk[0] == 3 and not blk[6] & CONT] == [1, 512]
     assert fresh_period(bs) == 511
     assert py_plan(frames, 8, seg)[0] == blocks
