@@ -252,6 +252,66 @@ lz4b200_status lz4b200_decompress_batch_host_with_dict(lz4b200_ctx *ctx,
     uint8_t *out, const uint64_t *out_off, const uint32_t *out_cap,
     uint32_t *out_len, int32_t *status, uint64_t *err_expected, size_t nblocks);
 
+/* ---- many size-prepended blocks, DEVICE pointers ----------------------------------------------------------------------
+ * A record is what block::compress_prepend_size writes: the input's length as a u32 LE word, then its block
+ * (src/block/compress.rs:673-675, src/block/mod.rs:151-157).  Every array lives in device memory.  Argument errors return
+ * INVALID_ARGUMENT before anything is enqueued, every output untouched: a null ctx or d_rec_off / d_out_off; with a
+ * non-empty batch a null input, descriptor or per-record array, or a null d_out with out_cap > 0; a count above
+ * UINT32_MAX; a null dictionary with dict_len > 0.  An empty batch writes 0 to d_rec_off[0] / d_out_off[0] and nothing
+ * else.  Otherwise the work is enqueued on `stream` and the call returns without synchronising (a call larger than any
+ * before it on the context first grows the context's scratch, and CUDA may synchronise while it frees and allocates).
+ * Like every device call, calls on one context must be ordered on one stream: they share the context's ticket counters
+ * and scratch.  d_in, d_out and the dictionary may have any alignment; d_out's bytes past the last written record are
+ * not written. */
+
+/* block::compress_prepend_size — src/block/compress.rs:673-675 — for each of many blocks, the records packed back to
+ * back.  Block b is d_in[in_off[b], in_off[b] + in_len[b]), compressed as the block API does (every block FRESH).
+ * Record b is exactly the bytes lz4b200_compress_prepend_size writes for that input; d_rec_off[b] is its offset in
+ * d_out and d_rec_off[nblocks] the total the batch needs (d_rec_off has nblocks + 1 entries).
+ * d_status[b]: OK, or COMPRESS_OUTPUT_TOO_SMALL when
+ *   - in_len[b] > max_in_len: max_in_len is a host bound on every in_len; it sizes the scratch, one slot of
+ *     lz4b200_max_output_size(max_in_len) per block, and such a block's slot is too small.  Its record takes 0 bytes.
+ *   - the record does not fit: d_rec_off[b] + its length > out_cap.  Nothing of it is written, but its length counts in
+ *     d_rec_off, so d_rec_off[nblocks] is what to allocate.
+ * The kernel that compresses the blocks is the one lz4b200_compress_batch_device picks for the same batch and
+ * max_in_len. */
+lz4b200_status lz4b200_compress_prepend_size_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_in_off, const uint32_t *d_in_len, size_t nblocks, uint32_t max_in_len,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_rec_off, int32_t *d_status, void *stream);
+
+/* block::compress_prepend_size_with_dict — src/block/compress.rs:692-694 — the same with one dictionary shared by every
+ * block, normalised as lz4b200_compress_batch_device_with_dict does (ignored at <= 3 bytes, the last 64 KiB kept):
+ * record b is the bytes of lz4b200_compress_prepend_size_with_dict. */
+lz4b200_status lz4b200_compress_prepend_size_batch_device_with_dict(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_in_off, const uint32_t *d_in_len, size_t nblocks, uint32_t max_in_len,
+    const uint8_t *d_dict, size_t dict_len,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_rec_off, int32_t *d_status, void *stream);
+
+/* block::decompress_size_prepended — src/block/decompress.rs:496-499 — for each of many records, with no host
+ * synchronisation: the length words set the output layout on the device.  Record b is d_in[rec_off[b], rec_off[b] +
+ * rec_len[b]).  d_out_off[b] is the sum of the length words of records 0..b-1 (a record of fewer than 4 bytes counts 0)
+ * and d_out_off[nrec] the total (d_out_off has nrec + 1 entries).  Record b decodes into d_out + d_out_off[b] with a
+ * capacity of exactly its length word, the reference's Vec::with_capacity.  d_status[b], d_out_len[b] and
+ * d_err_expected[b] (may be NULL) are the status, *written and *err_expected lz4b200_decompress_size_prepended returns
+ * for those bytes (err_actual is the length word), and the decoded bytes are the same:
+ *   - fewer than 4 bytes: DEC_EXPECTED_ANOTHER_BYTE (src/block/mod.rs:152);
+ *   - a region that ends past out_cap: INVALID_ARGUMENT (the one-record call's cap < size rule); nothing is written.
+ * Bytes of a region past d_out_len[b] are what lz4b200_decompress_batch_device leaves there: a decoded record leaves
+ * them untouched, a record that fails may leave there bytes it decoded before the error.  They are not zeroed (the host
+ * calls zero them).  The kernel that decodes is the one lz4b200_decompress_batch_device picks for nrec blocks. */
+lz4b200_status lz4b200_decompress_size_prepended_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_rec_off, const uint32_t *d_rec_len, size_t nrec,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_out_off, uint32_t *d_out_len,
+    int32_t *d_status, uint64_t *d_err_expected, void *stream);
+
+/* block::decompress_size_prepended_with_dict — src/block/decompress.rs:522-528 — the same with one dictionary shared by
+ * every record (the last 64 KiB kept, as lz4b200_decompress_batch_device_with_dict does). */
+lz4b200_status lz4b200_decompress_size_prepended_batch_device_with_dict(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_rec_off, const uint32_t *d_rec_len, size_t nrec,
+    const uint8_t *d_dict, size_t dict_len,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_out_off, uint32_t *d_out_len,
+    int32_t *d_status, uint64_t *d_err_expected, void *stream);
+
 /* ---- frame format (encoder: independent blocks; decoder: independent and linked) -------------
  * FrameInfo — src/frame/header.rs:130-192. */
 typedef struct lz4b200_frame_info {

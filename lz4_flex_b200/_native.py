@@ -140,6 +140,10 @@ SIGNATURES = {
     "lz4b200_decompress_batch_device_with_dict": (_i32, [_vp] * 5 + [_sz] + [_vp] * 6 + [_sz, _vp]),
     "lz4b200_compress_batch_host_with_dict": (_i32, [_vp] * 5 + [_sz, _vp, _sz] + [_vp] * 3 + [_sz]),
     "lz4b200_decompress_batch_host_with_dict": (_i32, [_vp] * 5 + [_sz] + [_vp] * 6 + [_sz]),
+    "lz4b200_compress_prepend_size_batch_device": (_i32, [_vp] * 4 + [_sz, _u32, _vp, _sz] + [_vp] * 3),
+    "lz4b200_compress_prepend_size_batch_device_with_dict": (_i32, [_vp] * 4 + [_sz, _u32, _vp, _sz, _vp, _sz] + [_vp] * 3),
+    "lz4b200_decompress_size_prepended_batch_device": (_i32, [_vp] * 4 + [_sz, _vp, _sz] + [_vp] * 5),
+    "lz4b200_decompress_size_prepended_batch_device_with_dict": (_i32, [_vp] * 4 + [_sz, _vp, _sz, _vp, _sz] + [_vp] * 5),
     "lz4b200_frame_bound": (_sz, [_sz, C.POINTER(FrameInfoC)]),
     "lz4b200_frame_compress": (_i32, [_vp, _vp, _sz, C.POINTER(FrameInfoC), _sz, _vp, _sz, _psz]),
     "lz4b200_frame_compress_device": (_i32, [_vp, _vp, _sz, C.POINTER(FrameInfoC), _sz, _vp, _sz, _vp, _vp]),

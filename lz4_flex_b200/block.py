@@ -468,3 +468,150 @@ class DeviceBatch:
             self.status.data_ptr(), self.expected.data_ptr(), self.nblocks, s)
         if st != 0:
             _raise(ctx, st)
+
+
+# ---- many size-prepended records, device memory ----------------------------------------------------------------
+
+def _device_u32(v, device):
+    """u32 values as a CUDA int32 tensor with the same bits."""
+    import torch
+    if isinstance(v, torch.Tensor):
+        return v.to(device=device).reshape(-1).to(torch.int32).contiguous()
+    return torch.from_numpy(np.asarray(v, dtype=np.int64).reshape(-1).astype(np.uint32).view(np.int32)).to(device)
+
+
+def _device_dict(ext_dict, device):
+    """(pointer, length, keepalive) of a dictionary given as a CUDA uint8 tensor or host bytes (uploaded)."""
+    import torch
+    if ext_dict is None:
+        return None, 0, None
+    if isinstance(ext_dict, torch.Tensor):
+        from .frame import _device_u8
+        _device_u8(ext_dict, "ext_dict")
+        d = ext_dict
+    else:
+        d = torch.from_numpy(_as_u8(ext_dict).copy()).to(device)
+    return (d.data_ptr() if d.numel() else None), d.numel(), d
+
+
+def _keep_for(stream, device, *tensors):
+    """Temporaries made on torch's stream and read by work on another `stream` stay allocated until that work is done."""
+    import torch
+    if stream is not None:
+        ext = torch.cuda.ExternalStream(stream, device=device)
+        for t in tensors:
+            if t is not None:
+                t.record_stream(ext)
+
+
+def _on_stream(stream, device):
+    import contextlib
+    import torch
+    return contextlib.nullcontext() if stream is None else torch.cuda.stream(torch.cuda.ExternalStream(stream, device=device))
+
+
+def compress_prepend_size_device(d_in, offsets, lengths, out=None, ext_dict=None, ctx: Context | None = None,
+                                 stream: int | None = None):
+    """compress_prepend_size() for each of many inputs in device memory, in one call
+    (lz4b200_compress_prepend_size_batch_device, or its _with_dict form when ext_dict is given: a CUDA uint8 tensor or
+    host bytes shared by every input).  Input i is d_in[offsets[i]:offsets[i] + lengths[i]]; record i, the bytes
+    compress_prepend_size() (or compress_prepend_size_with_dict()) gives for it, is out[rec_off[i]:rec_off[i + 1]],
+    records back to back from out[0].  `out` is a contiguous 1-D torch CUDA uint8 tensor; None allocates the bound,
+    the sum of 4 + get_maximum_output_size(length).  The lengths are read on the host (they bound the scratch and the
+    output), so a CUDA tensor of lengths is copied back first.  The work is enqueued on torch's current stream (or
+    `stream`) and the call returns without synchronising.  Returns (out, rec_off, status): CUDA tensors, rec_off int64
+    with len(lengths) + 1 entries (rec_off[-1] is the total the batch needs), status int32 per record, 0 or 1
+    (CompressOutputTooSmall: the record does not fit in `out` and was not written).  Raises on argument errors."""
+    import torch
+    from .frame import _device_i64, _device_u8
+    _device_u8(d_in, "d_in")
+    ctx = ctx or default_context()
+    dev = d_in.device
+    lens = (lengths.cpu().numpy() if isinstance(lengths, torch.Tensor) else np.asarray(lengths)).astype(np.int64).reshape(-1)
+    n = lens.size
+    if n and (lens.min() < 0 or lens.max() > 0xFFFFFFFF):
+        raise ValueError("lengths must be in [0, 2**32)")
+    if not isinstance(offsets, torch.Tensor):
+        o = np.asarray(offsets, dtype=np.int64).reshape(-1)
+        if o.size == n and n and (o.min() < 0 or int((o + lens).max()) > d_in.numel()):
+            raise ValueError("an input runs past the end of d_in")
+    offs = _device_i64(offsets, dev, "offsets")
+    if offs.numel() != n:
+        raise ValueError("offsets and lengths differ in length")
+    d_lens = _device_u32(lens, dev)
+    if out is None:
+        out = torch.empty(int(24 * n + (lens * 110 // 100).sum()), dtype=torch.uint8, device=dev)
+    _device_u8(out, "out")
+    dp, dn, keep = _device_dict(ext_dict, dev)
+    rec_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    src = d_in if d_in.numel() else torch.zeros(1, dtype=torch.uint8, device=dev)
+    args = (ctx.handle, src.data_ptr(), offs.data_ptr(), d_lens.data_ptr(), n, int(lens.max()) if n else 0)
+    tail = (out.data_ptr() if out.numel() else None, out.numel(), rec_off.data_ptr(), status.data_ptr(), s)
+    L = _native.lib()
+    if ext_dict is None:
+        st = L.lz4b200_compress_prepend_size_batch_device(*args, *tail)
+    else:
+        st = L.lz4b200_compress_prepend_size_batch_device_with_dict(*args, dp, dn, *tail)
+    if st != 0:
+        _raise(ctx, st)
+    _keep_for(stream, dev, offs, d_lens, keep)
+    return out, rec_off, status
+
+
+def decompress_size_prepended_device(d_in, rec_off, rec_len, out=None, ext_dict=None, ctx: Context | None = None,
+                                     stream: int | None = None):
+    """decompress_size_prepended() for each of many records in device memory, in one call
+    (lz4b200_decompress_size_prepended_batch_device, or its _with_dict form when ext_dict is given).  Record i is
+    d_in[rec_off[i]:rec_off[i] + rec_len[i]] (int tensors or sequences); it decodes into out[out_off[i]:], with room for
+    exactly its length word, and out_off is the running sum of the length words.  With `out` given the work is enqueued
+    on torch's current stream (or `stream`) and the call returns without synchronising.  With out=None the call first
+    runs with no output room, which decodes nothing, and reads the total back: that is a synchronise, the only one.
+    Returns (out, out_off, out_len, status, err_expected) as CUDA tensors: out_off int64 with len(rec_off) + 1 entries,
+    then per record the decoded length (int32), the status of the one-record call (int32: 0, a DecompressError code,
+    or 200 when the record's region runs past the end of `out`) and OutputTooSmall's `expected` (int64).  Records are
+    not raised on one by one (that would need a synchronise); argument errors raise."""
+    import torch
+    from .frame import _device_i64, _device_u8
+    _device_u8(d_in, "d_in")
+    ctx = ctx or default_context()
+    dev = d_in.device
+    offs, lens = _device_i64(rec_off, dev, "rec_off"), _device_u32(rec_len, dev)
+    n = offs.numel()
+    if lens.numel() != n:
+        raise ValueError("rec_off and rec_len differ in length")
+    if out is not None:
+        _device_u8(out, "out")
+    dp, dn, keep = _device_dict(ext_dict, dev)
+    out_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    out_len = torch.empty(n, dtype=torch.int32, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    expected = torch.empty(n, dtype=torch.int64, device=dev)
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    src = d_in if d_in.numel() else torch.zeros(1, dtype=torch.uint8, device=dev)
+    L = _native.lib()
+
+    def call(o):
+        head = (ctx.handle, src.data_ptr(), offs.data_ptr(), lens.data_ptr(), n)
+        tail = (o.data_ptr() if o is not None and o.numel() else None, o.numel() if o is not None else 0,
+                out_off.data_ptr(), out_len.data_ptr(), status.data_ptr(), expected.data_ptr(), s)
+        if ext_dict is None:
+            st = L.lz4b200_decompress_size_prepended_batch_device(*head, *tail)
+        else:
+            st = L.lz4b200_decompress_size_prepended_batch_device_with_dict(*head, dp, dn, *tail)
+        if st != 0:
+            _raise(ctx, st)
+
+    if out is None:
+        call(None)
+        with _on_stream(stream, dev):
+            total = int(out_off[n].item())
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    call(out)
+    _keep_for(stream, dev, offs, lens, keep)
+    return out, out_off, out_len, status, expected

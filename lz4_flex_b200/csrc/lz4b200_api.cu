@@ -148,6 +148,89 @@ __global__ void make_uniform_desc_kernel(uint64_t total_len, uint32_t block, uin
     flags[i] = (uint8_t)(LZ4B200_BLOCK_HASH5_ALWAYS | (fresh ? 0u : LZ4B200_BLOCK_CONT));
 }
 
+// ---- many size-prepended blocks (lz4b200_compress_prepend_size_batch_device & co) ---------------------------------------
+// A record is the input's length as a u32 LE word followed by its block (compress.rs:673-675, block/mod.rs:151-157).
+
+// The compressor's arguments, one thread per block: block b's slot is b x `slot` bytes.  A block longer than max_in_len
+// goes in empty with no room, which every encoder reports as COMPRESS_OUTPUT_TOO_SMALL (given its real length, the
+// encoder of small blocks would skip it and leave its status unwritten when max_in_len keeps the other one from running).
+__global__ void __launch_bounds__(128) prepend_desc_kernel(const uint32_t *in_len, uint32_t n, uint32_t max_in_len,
+                                                           uint32_t slot, uint32_t *len, uint64_t *out_off, uint32_t *out_cap)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    const bool fits = in_len[b] <= max_in_len;
+    len[b] = fits ? in_len[b] : 0u;
+    out_off[b] = (uint64_t)b * slot;
+    out_cap[b] = fits ? slot : 0u;
+}
+
+// Record sizes for the scan: the length word and the block, nothing for a block the encoder refused.
+__global__ void __launch_bounds__(128) prepend_size_kernel(const uint32_t *out_len, const int32_t *status, uint32_t n,
+                                                           uint32_t *size)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < n) size[b] = status[b] == LZ4B200_OK ? 4u + out_len[b] : 0u;
+}
+
+// A record that ends past out_cap fails and is not written.  The others get their length word here and their block from
+// the gather (dst, glen); the gather's own prefix word is written unconditionally, so it cannot skip a record.
+__global__ void __launch_bounds__(128) prepend_place_kernel(const uint32_t *in_len, const uint32_t *out_len,
+                                                            const uint64_t *rec_off, uint32_t n, uint64_t out_cap,
+                                                            uint8_t *out, int32_t *status, uint64_t *dst, uint32_t *glen)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    const uint64_t o = rec_off[b];
+    bool live = status[b] == LZ4B200_OK;
+    if (live && o + 4u + out_len[b] > out_cap) {
+        status[b] = LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
+        live = false;
+    }
+    dst[b] = o + 4u;
+    glen[b] = live ? out_len[b] : 0u;
+    if (live)
+        for (int i = 0; i < 4; i++) out[o + i] = (uint8_t)(in_len[b] >> (8 * i));
+}
+
+// Each record's length word, read a byte at a time (records start anywhere), is its output size; a record of fewer than
+// 4 bytes has none and takes no output.
+__global__ void __launch_bounds__(128) prepended_size_kernel(const uint8_t *in, const uint64_t *rec_off,
+                                                             const uint32_t *rec_len, uint32_t n, uint32_t *size)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    const uint8_t *p = in + rec_off[b];
+    size[b] = rec_len[b] < 4u ? 0u
+                              : (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
+}
+
+// The decoder's arguments: the block after the length word, decoded in place at out_off[b] with exactly the length word as
+// capacity (the reference's Vec::with_capacity).  A record of fewer than 4 bytes goes in empty, for which the decoder
+// reports DEC_EXPECTED_ANOTHER_BYTE as the one-record call does; so does a record whose region ends past out_cap, which
+// is flagged for prepended_status_kernel.
+__global__ void __launch_bounds__(128) prepended_args_kernel(const uint64_t *rec_off, const uint32_t *rec_len,
+                                                             const uint32_t *size, const uint64_t *out_off, uint32_t n,
+                                                             uint64_t out_cap, uint64_t *in_off, uint32_t *in_len,
+                                                             uint32_t *cap, uint8_t *misfit)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    const uint32_t len = rec_len[b];
+    const bool fits = out_off[b] + size[b] <= out_cap, decode = len >= 4u && fits;
+    in_off[b] = rec_off[b] + 4u;
+    in_len[b] = decode ? len - 4u : 0u;
+    cap[b] = decode ? size[b] : 0u;
+    misfit[b] = len >= 4u && !fits;
+}
+
+// After the decoder: the one-record call's `cap < want` rule for the records flagged above.
+__global__ void __launch_bounds__(128) prepended_status_kernel(const uint8_t *misfit, uint32_t n, int32_t *status)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < n && misfit[b]) status[b] = LZ4B200_INVALID_ARGUMENT;
+}
+
 // ---- device-resident frame decoder (lz4b200_frame_decompress_next_device) ----------------------------------------------
 
 // One thread walks the frame at `in` (fw::frame_walk, the same code the host path runs), resuming from *w and
@@ -1030,6 +1113,22 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
     return LZ4B200_OK;
 }
 
+// The reference keeps only the last WINDOW_SIZE bytes of a dictionary (init_dict, compress.rs:571-575) and drops
+// dictionaries of <= 3 bytes (compress_into_vec_with_dict, compress.rs:626-628).
+void normalize_dict(const uint8_t *&dict, size_t &dict_len, bool for_compress)
+{
+    if (!dict || (for_compress && dict_len <= 3)) { dict = nullptr; dict_len = 0; return; }
+    if (dict_len > 65536) { dict += dict_len - 65536; dict_len = 65536; }
+}
+
+// The batch's dictionary, normalised, in a.
+void set_dict(BatchArgs &a, const uint8_t *dict, size_t dict_len, bool for_compress)
+{
+    normalize_dict(dict, dict_len, for_compress);
+    a.dict = dict;
+    a.dict_len = (uint32_t)dict_len;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1286,10 +1385,7 @@ lz4b200_status lz4b200_compress_batch_device_with_dict(lz4b200_ctx *ctx, const u
     DeviceGuard guard(ctx->device);
     BatchArgs a{d_in, d_in_off, d_in_len, nullptr, d_out, d_out_off, d_out_cap, d_out_len, d_status, nullptr,
                 (uint32_t)nblocks, nullptr};
-    if (dict_len > 3) {
-        if (dict_len > 65536) { d_dict += dict_len - 65536; dict_len = 65536; }
-        a.dict = d_dict; a.dict_len = (uint32_t)dict_len;
-    }
+    set_dict(a, d_dict, dict_len, true);
     return launch_compress(ctx, a, max_in_len, (cudaStream_t)stream);
 }
 
@@ -1306,11 +1402,144 @@ lz4b200_status lz4b200_decompress_batch_device_with_dict(lz4b200_ctx *ctx, const
     DeviceGuard guard(ctx->device);
     BatchArgs a{d_in, d_in_off, d_in_len, nullptr, d_out, d_out_off, d_out_cap, d_out_len, d_status, d_err_expected,
                 (uint32_t)nblocks, nullptr};
-    if (dict_len) {
-        if (dict_len > 65536) { d_dict += dict_len - 65536; dict_len = 65536; }
-        a.dict = d_dict; a.dict_len = (uint32_t)dict_len;
-    }
+    set_dict(a, d_dict, dict_len, false);
     return launch_decompress(ctx, a, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// lz4b200_compress_prepend_size_batch_device(_with_dict): compress every block into a slot of max_output_size(max_in_len)
+// bytes with the block API's launch, scan the record sizes into rec_off, then write each record that fits at its offset.
+lz4b200_status compress_prepend_size_batch(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
+                                           const uint32_t *d_in_len, size_t nblocks, uint32_t max_in_len,
+                                           const uint8_t *d_dict, size_t dict_len, uint8_t *d_out, size_t out_cap,
+                                           uint64_t *d_rec_off, int32_t *d_status, void *stream)
+{
+    if (!ctx || !d_rec_off || nblocks > 0xffffffffull || (!d_dict && dict_len)) return LZ4B200_INVALID_ARGUMENT;
+    if (nblocks && (!d_in || !d_in_off || !d_in_len || !d_status || (!d_out && out_cap))) return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (nblocks == 0) {
+        CTX_CUDA(ctx, cudaMemsetAsync(d_rec_off, 0, 8, s));
+        return LZ4B200_OK;
+    }
+    const uint32_t n = (uint32_t)nblocks, grid = (n + 127) / 128;
+    const uint32_t slot = (uint32_t)std::min<size_t>(lz4b200_max_output_size(max_in_len), 0xffffffffu);
+    CTX_CUDA(ctx, ctx->d_slots.reserve((size_t)n * slot + 16));
+    CTX_CUDA(ctx, ctx->d_in_len.reserve(n)); CTX_CUDA(ctx, ctx->d_out_off.reserve(n));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(n)); CTX_CUDA(ctx, ctx->d_out_len.reserve(n));
+    CTX_CUDA(ctx, ctx->d_seg_size.reserve(n)); CTX_CUDA(ctx, ctx->d_gdst.reserve(n));
+    CTX_CUDA(ctx, ctx->d_payload_len.reserve(n));
+    prepend_desc_kernel<<<grid, 128, 0, s>>>(d_in_len, n, max_in_len, slot, ctx->d_in_len.p, ctx->d_out_off.p,
+                                             ctx->d_out_cap.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    BatchArgs a{d_in, d_in_off, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p, ctx->d_out_cap.p,
+                ctx->d_out_len.p, d_status, nullptr, n, nullptr};
+    set_dict(a, d_dict, dict_len, true);
+    const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
+    if (st != LZ4B200_OK) return st;
+    prepend_size_kernel<<<grid, 128, 0, s>>>(ctx->d_out_len.p, d_status, n, ctx->d_seg_size.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, d_rec_off, n);
+    CTX_CUDA(ctx, cudaGetLastError());
+    prepend_place_kernel<<<grid, 128, 0, s>>>(d_in_len, ctx->d_out_len.p, d_rec_off, n, out_cap, d_out, d_status,
+                                              ctx->d_gdst.p, ctx->d_payload_len.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    GatherArgs g{ctx->d_slots.p, nullptr, ctx->d_out_off.p, nullptr, ctx->d_payload_len.p, nullptr, nullptr, nullptr,
+                 d_out, ctx->d_gdst.p, n};
+    gather_segments_kernel<<<std::min<uint32_t>(std::max<uint32_t>(n, (uint32_t)ctx->sm_count * 2),
+                                                (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+// lz4b200_decompress_size_prepended_batch_device(_with_dict): the length words give the output layout on the device, so
+// every record decodes in place into d_out with the block API's launch, and nothing returns to the host.
+lz4b200_status decompress_size_prepended_batch(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_rec_off,
+                                               const uint32_t *d_rec_len, size_t nrec, const uint8_t *d_dict,
+                                               size_t dict_len, uint8_t *d_out, size_t out_cap, uint64_t *d_out_off,
+                                               uint32_t *d_out_len, int32_t *d_status, uint64_t *d_err_expected,
+                                               void *stream)
+{
+    if (!ctx || !d_out_off || nrec > 0xffffffffull || (!d_dict && dict_len)) return LZ4B200_INVALID_ARGUMENT;
+    if (nrec && (!d_in || !d_rec_off || !d_rec_len || !d_out_len || !d_status || (!d_out && out_cap)))
+        return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (nrec == 0) {
+        CTX_CUDA(ctx, cudaMemsetAsync(d_out_off, 0, 8, s));
+        return LZ4B200_OK;
+    }
+    const uint32_t n = (uint32_t)nrec, grid = (n + 127) / 128;
+    CTX_CUDA(ctx, ctx->d_seg_size.reserve(n)); CTX_CUDA(ctx, ctx->d_in_off.reserve(n));
+    CTX_CUDA(ctx, ctx->d_in_len.reserve(n)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(n));
+    CTX_CUDA(ctx, ctx->d_pick.reserve(n));
+    prepended_size_kernel<<<grid, 128, 0, s>>>(d_in, d_rec_off, d_rec_len, n, ctx->d_seg_size.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, d_out_off, n);
+    CTX_CUDA(ctx, cudaGetLastError());
+    prepended_args_kernel<<<grid, 128, 0, s>>>(d_rec_off, d_rec_len, ctx->d_seg_size.p, d_out_off, n, out_cap,
+                                               ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_pick.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, d_out, d_out_off, ctx->d_out_cap.p, d_out_len, d_status,
+                d_err_expected, n, nullptr};
+    set_dict(a, d_dict, dict_len, false);
+    const lz4b200_status st = launch_decompress(ctx, a, s);
+    if (st != LZ4B200_OK) return st;
+    prepended_status_kernel<<<grid, 128, 0, s>>>(ctx->d_pick.p, n, d_status);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+// ---- many size-prepended blocks, device pointers --------------------------------------------------------------------
+
+lz4b200_status lz4b200_compress_prepend_size_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                          const uint32_t *d_in_len, size_t nblocks, uint32_t max_in_len,
+                                                          uint8_t *d_out, size_t out_cap, uint64_t *d_rec_off,
+                                                          int32_t *d_status, void *stream)
+{
+    return compress_prepend_size_batch(ctx, d_in, d_in_off, d_in_len, nblocks, max_in_len, nullptr, 0, d_out, out_cap,
+                                       d_rec_off, d_status, stream);
+}
+
+lz4b200_status lz4b200_compress_prepend_size_batch_device_with_dict(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                                    const uint64_t *d_in_off, const uint32_t *d_in_len,
+                                                                    size_t nblocks, uint32_t max_in_len,
+                                                                    const uint8_t *d_dict, size_t dict_len,
+                                                                    uint8_t *d_out, size_t out_cap, uint64_t *d_rec_off,
+                                                                    int32_t *d_status, void *stream)
+{
+    return compress_prepend_size_batch(ctx, d_in, d_in_off, d_in_len, nblocks, max_in_len, d_dict, dict_len, d_out,
+                                       out_cap, d_rec_off, d_status, stream);
+}
+
+lz4b200_status lz4b200_decompress_size_prepended_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                              const uint64_t *d_rec_off, const uint32_t *d_rec_len,
+                                                              size_t nrec, uint8_t *d_out, size_t out_cap,
+                                                              uint64_t *d_out_off, uint32_t *d_out_len, int32_t *d_status,
+                                                              uint64_t *d_err_expected, void *stream)
+{
+    return decompress_size_prepended_batch(ctx, d_in, d_rec_off, d_rec_len, nrec, nullptr, 0, d_out, out_cap, d_out_off,
+                                           d_out_len, d_status, d_err_expected, stream);
+}
+
+lz4b200_status lz4b200_decompress_size_prepended_batch_device_with_dict(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                                        const uint64_t *d_rec_off,
+                                                                        const uint32_t *d_rec_len, size_t nrec,
+                                                                        const uint8_t *d_dict, size_t dict_len,
+                                                                        uint8_t *d_out, size_t out_cap,
+                                                                        uint64_t *d_out_off, uint32_t *d_out_len,
+                                                                        int32_t *d_status, uint64_t *d_err_expected,
+                                                                        void *stream)
+{
+    return decompress_size_prepended_batch(ctx, d_in, d_rec_off, d_rec_len, nrec, d_dict, dict_len, d_out, out_cap,
+                                           d_out_off, d_out_len, d_status, d_err_expected, stream);
 }
 
 // ---- host batch entry points --------------------------------------------------------------------
@@ -1414,14 +1643,6 @@ static void pipeline_destroy(void *vp)
     if (p->h_seg) cudaFreeHost(p->h_seg);
     if (p->h_status) cudaFreeHost(p->h_status);
     delete p;
-}
-
-// The reference keeps only the last WINDOW_SIZE bytes of a dictionary (init_dict, compress.rs:571-575) and drops
-// dictionaries of <= 3 bytes (compress_into_vec_with_dict, compress.rs:626-628).
-static void normalize_dict(const uint8_t *&dict, size_t &dict_len, bool for_compress)
-{
-    if (!dict || (for_compress && dict_len <= 3)) { dict = nullptr; dict_len = 0; return; }
-    if (dict_len > 65536) { dict += dict_len - 65536; dict_len = 65536; }
 }
 
 static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *in, const uint64_t *in_off,
