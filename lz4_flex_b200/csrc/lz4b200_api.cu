@@ -1339,6 +1339,21 @@ void lz4b200_xxh32_update(lz4b200_xxh32_state *st, const uint8_t *data, size_t n
 
 uint32_t lz4b200_xxh32_digest(const lz4b200_xxh32_state *st) { return fw::xxh32_digest(*st); }
 
+#ifdef LZ4B200_ENC_PROFILE
+// Development build only: copies the matcher's phase counters (lz4b200::EncProfSlot order) of the current device to
+// out[0..16) and, if reset != 0, clears them.  Synchronises the device.
+int lz4b200_enc_profile_read(uint64_t *out, int reset)
+{
+    if (cudaDeviceSynchronize() != cudaSuccess) return LZ4B200_CUDA_ERROR;
+    if (cudaMemcpyFromSymbol(out, lz4b200::g_enc_profile, sizeof(lz4b200::g_enc_profile)) != cudaSuccess) return LZ4B200_CUDA_ERROR;
+    if (reset) {
+        static const unsigned long long zero[lz4b200::kEncProfSlots] = {};
+        if (cudaMemcpyToSymbol(lz4b200::g_enc_profile, zero, sizeof(zero)) != cudaSuccess) return LZ4B200_CUDA_ERROR;
+    }
+    return LZ4B200_OK;
+}
+#endif
+
 // ---- device batch entry points ----------------------------------------------------------------
 
 lz4b200_status lz4b200_compress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,

@@ -54,6 +54,53 @@ constexpr uint32_t kRingBytes = ENC_WINDOW ? kWinBytes : 0;   // shared memory a
 constexpr uint32_t kExitBlock = 0xffffffffu;
 constexpr uint32_t kSmallLit = 24;            // literal runs up to this length are copied by the owning lane
 
+#ifdef LZ4B200_ENC_PROFILE
+// Development build only (tests/dev/enc_phase_probe.py; neither library defines it): the matcher's clock64() cycles per phase
+// of match_block_view and a few event counts, kept per block in registers and added to g_enc_profile by lane 0 when the
+// block ends.  The cycles of a phase run from the end of the previous phase to the first warp-wide step that consumes its
+// results, so a load's latency is charged to the phase that waits for it.
+enum EncProfSlot : int {
+    kPhProbe,      // probe batch: re-insert, input and table loads, candidate fetch, hit ballot
+    kPhResolve,    // in-batch slot collisions (shuffles / match.any) and the forwarded candidates
+    kPhCommit,     // table writes of the executed probes, winner broadcast, next batch set-up
+    kPhExtend,     // backward and forward extension
+    kPhPush,       // tuple hand-off, including the wait for a free ring half
+    kPhSetup,      // table reset and the first insert of a block
+    kCtSeq,        // sequences (tuples with a match)
+    kCtBatch,      // probe batches
+    kCtNoBack,     // sequences without literals before the match (no backward round)
+    kCtShort,      // sequences with no backward round whose forward mismatch is within 8 bytes of the match start + 4
+    kCtLong,       // sequences that needed a second forward round (match longer than 36 bytes)
+    kCtBlocks,     // blocks
+    kEncProfSlots = 16
+};
+__device__ unsigned long long g_enc_profile[kEncProfSlots];
+struct EncProfile {
+    uint64_t t;
+    uint32_t c[kEncProfSlots];
+    __device__ __forceinline__ void start()
+    {
+#pragma unroll
+        for (int i = 0; i < kEncProfSlots; i++) c[i] = 0;
+        t = clock64();
+    }
+    __device__ __forceinline__ void phase(int i) { const uint64_t now = clock64(); c[i] += (uint32_t)(now - t); t = now; }
+    __device__ __forceinline__ void count(int i, bool on = true) { c[i] += on ? 1u : 0u; }
+    __device__ __forceinline__ void flush(uint32_t lane)
+    {
+        c[kCtBlocks]++;
+        if (lane == 0) {
+#pragma unroll
+            for (int i = 0; i < kEncProfSlots; i++)
+                if (c[i]) atomicAdd(g_enc_profile + i, (unsigned long long)c[i]);
+        }
+    }
+};
+#define ENC_PROF(x) prof.x
+#else
+#define ENC_PROF(x) ((void)0)
+#endif
+
 // mbarrier hand-off (shared-memory barrier objects; named barriers would cost 16 hardware barriers per CTA
 // and cap the resident CTAs).  One arrival per phase, from lane 0 of the signalling warp, after its writes.
 __device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -321,8 +368,13 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
     static_assert(!kTag || (kGT && sizeof(TabT) == 4), "tagged entries: global u32 tables");
     constexpr uint32_t kInvalid = kTag ? 0xffffffffu : TabTraits<TabT>::kInvalid;
     const uint32_t lt_mask = (1u << lane) - 1u;
+#ifdef LZ4B200_ENC_PROFILE
+    EncProfile prof;
+#endif
+    ENC_PROF(start());
     if (n < 13) {                                               // compress.rs:343-346
         pr.push_final(0, n, lane);
+        ENC_PROF(flush(lane));
         return;
     }
     view.advance(0u);
@@ -353,6 +405,7 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
         cur = 1;
         __syncwarp();
     }
+    ENC_PROF(phase(kPhSetup));
 
     for (;;) {                                                  // one sequence per iteration
 #if ENC_WINDOW
@@ -363,6 +416,7 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
         uint32_t base = cur, stride = 1, width = ENC_FIRST_WIDTH, cand, mpos;
         bool in_win = ENC_WINDOW != 0;                          // first batch: probe bytes come from the ring
         for (;;) {                                              // probe batches: compress.rs:373-439
+            ENC_PROF(count(kCtBatch));
             view.advance(base);
             const uint32_t p = base + lane * stride;
             const bool act = lane < width;
@@ -412,6 +466,7 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
             }
             uint32_t hits = __ballot_sync(kFull, hit);
             const uint32_t terms = (base + 31u * stride > last_probe) ? __ballot_sync(kFull, term) : 0u;   // uniform: only near the block's end
+            ENC_PROF(phase(kPhProbe));
             const uint32_t w0 = hits ? (uint32_t)__ffs(hits) - 1u : 32u;
             uint32_t same = 1u << lane;                         // lanes of this batch on my slot (incl. me)
             bool exact = w0 == 0u;
@@ -439,10 +494,13 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
                     hits = __ballot_sync(kFull, hit);
                 }
             }
+            ENC_PROF(phase(kPhResolve));
             const uint32_t win = hits ? (uint32_t)__ffs(hits) - 1u : 32u;
             const uint32_t tfirst = terms ? (uint32_t)__ffs(terms) - 1u : 32u;
             if (tfirst < win) {                                 // compress.rs:381-384: the rest is literals
                 pr.push_final(anchor, n, lane);
+                ENC_PROF(phase(kPhPush));
+                ENC_PROF(flush(lane));
                 return;
             }
             // commit the table writes of probes 0..win (last writer per slot wins)
@@ -457,6 +515,7 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
             }
 #endif
             __syncwarp();
+            ENC_PROF(phase(kPhCommit));
             if (win < 32u) {
                 mpos = base + win * stride;
                 cand = __shfl_sync(kFull, cnd, win);
@@ -521,7 +580,13 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
                 end += (uint32_t)__ffs(~__ballot_sync(kFull, ok)) - 1u;
             }
         }
+        ENC_PROF(phase(kPhExtend));
+        ENC_PROF(count(kCtSeq));
+        ENC_PROF(count(kCtNoBack, room == 0u));
+        ENC_PROF(count(kCtShort, room == 0u && kf < 8u));
+        ENC_PROF(count(kCtLong, kf == 32u));
         pr.push(anchor, mpos, dist, end, lane);
+        ENC_PROF(phase(kPhPush));
         anchor = cur = end;
         ri = true;
     }
@@ -1113,7 +1178,10 @@ lz4_compress_blocks_gtab(BatchArgs a, uint32_t *tickets, TabT *gtab)
     __shared__ uint32_t meta_s[kM * 8];
     __shared__ __align__(8) uint64_t bars_s[kM * 4];
     __shared__ EmitState st_s[kM];
-    const uint32_t warp = threadIdx.x >> 5, lane = lane_id();
+    // The warp index comes from a warp reduction, which writes a uniform register: with threadIdx.x >> 5 the compiler cannot
+    // tell that the role branches below are warp-uniform, and it then guards every shuffle, ballot and match.any of the
+    // matcher and the emitter with a divergence check and a collective-emulation fall-back (88 of them in this kernel).
+    const uint32_t warp = __reduce_max_sync(kFull, threadIdx.x >> 5), lane = lane_id();
     if (threadIdx.x < (uint32_t)kM * 4u) mbar_init(bars_s + threadIdx.x, 1u);
     __syncthreads();
     if (warp >= (uint32_t)kM) {
