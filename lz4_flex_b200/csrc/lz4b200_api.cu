@@ -488,10 +488,30 @@ __global__ void __launch_bounds__(128) frame_batch_tail_kernel(uint8_t *out, con
     if (f == n - 1) frame_off[n] = o;
 }
 
+// ---- the frame decoders' group pipeline ---------------------------------------------------------------------------------
+// Every frame decoder decodes a frame group by group through the same kernels: arguments, decode, resolve, gather,
+// content hash, digest (decode_group).  A group holds the blocks of one or more frames, described by one GroupFrame
+// each: the batch decoder's record walk fills one per frame, the group loop (decode_frame_blocks) one per group of a
+// frame.  Blocks are indexed frame after frame, the blocks of independent frames first and those of linked frames
+// after them.
+struct GroupFrame {
+    uint64_t in_off;                  // the frame's first byte is at src + in_off (unsigned: payload offsets add to it)
+    uint64_t out_off, out_cap;        // the group's output goes to out + out_off, at most out_cap bytes
+    uint64_t delivered;               // the frame's bytes that earlier groups delivered
+    const fw::FrameWalk *walk;        // the frame's walk
+    lz4b200_xxh32_state *content;     // the frame's content hash, carried from group to group (null: hashed by the host)
+    lz4b200_frame_result *result;
+    uint32_t base, nblocks;           // the group's descriptors of this frame: [base, base + nblocks)
+    uint32_t bad;                     // the first of them not delivered: the first to fail its checksum (kNoBlock: none),
+                                      // lowered by the resolve step to the first that fails to decode
+    uint8_t window;                   // 1: descriptor `base` is a linked window's stored pseudo-block, not output
+    uint8_t last;                     // the group ends the frame: the walk status and the EndMark rules apply
+};
+
 // ---- batch frame decoder (lz4b200_frame_decompress_batch_device) --------------------------------------------------------
 // Many independent frames per call.  Frame f is the one that starts at in + frame_off[f] in a region of frame_len[f]
-// bytes.  The host plans groups of whole frames from a count walk; per group, blocks are indexed frame after frame, the
-// blocks of independent frames first and those of linked frames after them (descriptor index `base` of a frame).
+// bytes.  The host plans groups of whole frames from a count walk; each group's frames are each one group of the
+// pipeline above.
 
 // Count walk, one thread per frame: the walk state, the count, and the block count per class (independent blocks at
 // nb2[f], linked at nb2[n + f]) for the descriptor scans.
@@ -529,13 +549,15 @@ __global__ void __launch_bounds__(128) frame_bound_kernel(const uint8_t *in, con
 }
 
 // Record walk of the group's frames [f0, f0 + gn), one thread per frame: each frame's descriptors at its base (from the
-// scans of the two block-count classes), and per block its frame and slot bytes.
+// scans of the two block-count classes), its block's frame, and its GroupFrame as one group ending the frame.
 __global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, const uint64_t *frame_off,
-                                                           const uint64_t *frame_len, uint32_t f0, uint32_t gn,
+                                                           const uint64_t *frame_len, const uint64_t *frame_out_off,
+                                                           const uint64_t *frame_out_cap, uint32_t f0, uint32_t gn,
                                                            const fw::FrameWalk *walks, const fw::FrameCount *counts,
                                                            const uint64_t *scan_ind, const uint64_t *scan_lnk,
-                                                           fw::FrameBlockDesc *desc, uint32_t *fbase, uint32_t *bframe,
-                                                           uint32_t *bslot, uint32_t *bad)
+                                                           fw::FrameBlockDesc *desc, uint32_t *bframe,
+                                                           lz4b200_xxh32_state *states, lz4b200_frame_result *results,
+                                                           GroupFrame *frames)
 {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= gn) return;
@@ -544,136 +566,148 @@ __global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, co
     const uint32_t base = (uint32_t)(c.linked ? scan_ind[gn] + scan_lnk[g] : scan_ind[g]);
     fw::FrameWalk w;
     const uint32_t nb = fw::frame_walk(in + frame_off[f], frame_len[f], w, desc + base, (uint32_t)c.nblocks);
-    for (uint32_t k = 0; k < nb; k++) {
-        bframe[base + k] = g;
-        bslot[base + k] = (uint32_t)fw::slot_bytes(fw::block_slot_cap(desc[base + k], walks[f].bs));
-    }
-    fbase[g] = base;
-    bad[g] = fw::kNoBlock;
+    for (uint32_t k = 0; k < nb; k++) bframe[base + k] = g;
+    GroupFrame p{};
+    p.in_off = frame_off[f];
+    p.out_off = frame_out_off[f];
+    p.out_cap = frame_out_cap[f];
+    p.walk = walks + f;
+    p.content = states + g;
+    p.result = results + f;
+    p.base = base;
+    p.nblocks = nb;
+    p.bad = fw::kNoBlock;
+    p.last = 1;
+    frames[g] = p;
 }
 
-// Block checksums, one thread per block of the group; bad[g] receives the first failing block of frame g.
-__global__ void __launch_bounds__(128) frame_batch_checksum_kernel(const uint8_t *in, const uint64_t *frame_off,
-                                                                   uint32_t f0, const fw::FrameWalk *walks,
-                                                                   const fw::FrameBlockDesc *desc, const uint32_t *fbase,
-                                                                   const uint32_t *bframe, uint32_t nb, uint32_t *bad)
+// Block checksums, one thread per block of the group; frames[g].bad receives the first failing block of frame g.
+__global__ void __launch_bounds__(128) frame_batch_checksum_kernel(const uint8_t *in, const fw::FrameBlockDesc *desc,
+                                                                   const uint32_t *bframe, uint32_t nb, GroupFrame *frames)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
-    const uint32_t g = bframe[b];
-    if (!(walks[f0 + g].flg & 0x10)) return;
-    if (!fw::block_checksum_ok(in + frame_off[f0 + g], desc[b])) atomicMin(bad + g, b - fbase[g]);
+    GroupFrame &p = frames[bframe[b]];
+    if (!(p.walk->flg & 0x10)) return;
+    if (!fw::block_checksum_ok(in + p.in_off, desc[b])) atomicMin(&p.bad, b - p.base);
 }
 
 // The decoder's arguments, one thread per block of the group: blocks at and past a frame's first bad block are not
 // decoded (in_len 0, cap 0, like a stored block) and nothing of theirs is delivered.  Linked blocks (index >= nind)
-// also get their chain start relative to the linked launch's first block.
-__global__ void __launch_bounds__(128) frame_batch_args_kernel(const uint64_t *frame_off, uint32_t f0,
-                                                               const fw::FrameWalk *walks, const fw::FrameBlockDesc *desc,
-                                                               const uint32_t *fbase, const uint32_t *bframe,
-                                                               const uint32_t *bad, uint32_t nb, uint32_t nind,
+// also get their chain start relative to the linked launch's first block.  slot[b]: the bytes of block b's slot.
+__global__ void __launch_bounds__(128) frame_batch_args_kernel(const GroupFrame *frames, const fw::FrameBlockDesc *desc,
+                                                               const uint32_t *bframe, uint32_t nb, uint32_t nind,
                                                                uint64_t *in_off, uint32_t *in_len, uint32_t *out_cap,
                                                                uint8_t *pick, uint32_t *link_first, uint32_t *stored_len,
-                                                               uint32_t *done)
+                                                               uint32_t *done, uint32_t *slot)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
-    const uint32_t g = bframe[b];
+    const GroupFrame &p = frames[bframe[b]];
     const fw::FrameBlockDesc d = desc[b];
-    const bool live = b - fbase[g] < bad[g], stored = fw::block_stored(d), decode = live && !stored;
-    in_off[b] = frame_off[f0 + g] + d.payload_off;
+    const uint64_t bs = p.walk->bs;
+    const bool live = b - p.base < p.bad, stored = fw::block_stored(d), decode = live && !stored;
+    in_off[b] = p.in_off + d.payload_off;
     in_len[b] = decode ? fw::block_len(d) : 0u;
-    out_cap[b] = decode ? (uint32_t)fw::block_decoded_cap(fw::block_len(d), walks[f0 + g].bs) : 0u;
+    out_cap[b] = decode ? (uint32_t)fw::block_decoded_cap(fw::block_len(d), bs) : 0u;
     pick[b] = decode ? 0 : 1;
+    slot[b] = (uint32_t)fw::slot_bytes(fw::block_slot_cap(d, bs));
     if (b >= nind) {
-        link_first[b] = fbase[g] - nind;
+        link_first[b] = p.base - nind;
         stored_len[b] = live && stored ? fw::block_len(d) : 0u;
         done[b] = 0;
     }
 }
 
-// One thread per frame of the group: the group loop's result for a frame that is one group (decode_frame_blocks, then
-// frame_decompress_next_impl's checks at the EndMark), and the gather of its delivered blocks.  hash[g] is set, and
-// states[g] reset, when the result still depends on the content checksum.
-__global__ void __launch_bounds__(128) frame_resolve_kernel(uint32_t f0, uint32_t gn, const fw::FrameWalk *walks,
-                                                            const fw::FrameCount *counts, const fw::FrameBlockDesc *desc,
-                                                            const uint32_t *fbase, const uint32_t *bad,
-                                                            const uint32_t *out_len, const int32_t *status,
-                                                            const uint64_t *expected, const uint32_t *blk_cap,
-                                                            const uint64_t *frame_out_off, const uint64_t *frame_out_cap,
-                                                            uint64_t *dst_off, uint32_t *glen, uint8_t *hash,
-                                                            lz4b200_xxh32_state *states, lz4b200_frame_result *results)
+// One warp per frame of the group: the frame's result after this group, and the gather of its delivered blocks.
+// The rules, in order: the first failing block in stream order ends the output; output past out_cap is OUTPUT_FULL
+// (nothing of the group delivered), checked before the decode error; then, in the group that ends the frame, the
+// walk's status and at the EndMark the content length (the digest kernel compares the content checksum).  hash[g] is
+// set when the group's output goes into the frame's content hash (if it has one), which is reset when the frame has
+// delivered nothing.  A warp, not a thread: the group loop's one frame may hold thousands of blocks.
+__global__ void __launch_bounds__(128) frame_resolve_kernel(GroupFrame *frames, uint32_t gn,
+                                                            const fw::FrameBlockDesc *desc, const uint32_t *out_len,
+                                                            const int32_t *status, const uint64_t *expected,
+                                                            const uint32_t *blk_cap, uint64_t *dst_off, uint32_t *glen,
+                                                            uint8_t *hash)
 {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= gn) return;
-    const uint32_t f = f0 + g, base = fbase[g], nrec = (uint32_t)counts[f].nblocks;
-    fw::FrameWalk w = walks[f];
-    if (bad[g] != fw::kNoBlock) fw::frame_walk_fail_block(w, desc[base + bad[g]], bad[g]);
-    const uint32_t nb = (uint32_t)w.nblocks;
+    const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
+    if (g >= gn) return;                                    // whole warps
+    const GroupFrame p = frames[g];
+    const uint32_t base = p.base, nrec = p.nblocks, end = min(nrec, p.bad);
+    uint32_t good = end;                                    // the first block of [window, end) that failed to decode
+    uint64_t total = 0;                                     // the delivered blocks' output, packed in stream order
+#pragma unroll 4
+    for (uint32_t k0 = 0; k0 < nrec; k0 += 32) {
+        const uint32_t k = k0 + lane, b = base + k;
+        const bool live = k >= p.window && k < end, stored = live && fw::block_stored(desc[b]);
+        const uint32_t m = __ballot_sync(kFull, live && !stored && status[b] != 0);
+        if (m && good == end) good = k0 + __ffs(m) - 1;
+        const uint32_t len = live && k < good ? (stored ? fw::block_len(desc[b]) : out_len[b]) : 0u;
+        uint64_t x = len;
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(kFull, x, d);
+            if (lane >= d) x += y;
+        }
+        if (k < nrec) { dst_off[b] = p.out_off + total + x - len; glen[b] = len; }
+        total += __shfl_sync(kFull, x, 31);
+    }
+    const bool full = total > p.out_cap;
+    if (full)
+        for (uint32_t k = lane; k < nrec; k += 32) glen[base + k] = 0;
+    if (lane) return;
+    fw::FrameWalk w = *p.walk;
+    if (p.bad != fw::kNoBlock) fw::frame_walk_fail_block(w, desc[base + p.bad], p.bad);
     lz4b200_frame_result r{};
     r.consumed = w.ip;
-    uint32_t good = nb;
-    uint64_t total = 0;
-    for (uint32_t k = 0; k < nrec; k++) {                   // the first failing block in stream order ends the output
-        const uint32_t b = base + k;
-        uint32_t len = 0;
-        if (k < good) {
-            if (fw::block_stored(desc[b])) len = fw::block_len(desc[b]);
-            else if (status[b] != 0) good = k;
-            else len = out_len[b];
-        }
-        dst_off[b] = frame_out_off[f] + total;
-        glen[b] = len;
-        total += len;
-    }
-    uint8_t h = 0;
-    if (total > frame_out_cap[f]) {                         // checked before the decode error, as the group loop does
+    r.written = p.delivered;
+    if (full) {
         r.status = LZ4B200_FRAME_OUTPUT_FULL;
-        for (uint32_t k = 0; k < nrec; k++) glen[base + k] = 0;
     } else {
-        r.written = total;
-        if (good < nb) {
+        r.written += total;
+        if (good < end) {
             const uint32_t b = base + good;
             r.status = LZ4B200_FRAME_DECOMPRESSION_ERROR;
             r.block_status = status[b];
             if (status[b] == LZ4B200_DEC_OUTPUT_TOO_SMALL) { r.err_expected = expected[b]; r.err_actual = blk_cap[b]; }
-        } else if (w.status != LZ4B200_OK) {
+            frames[g].bad = good - p.window;
+        } else if (p.last && w.status != LZ4B200_OK) {
             r.status = w.status;
-        } else if (w.closed) {
-            if (w.has_size && total != w.content_size) {
-                r.status = LZ4B200_FRAME_CONTENT_LENGTH;
-                r.err_expected = w.content_size;
-                r.err_actual = total;
-            } else if (w.has_checksum) {
-                h = 1;
-                fw::xxh32_reset(states[g], 0);
-            }
+        } else if (p.last && w.closed && w.has_size && r.written != w.content_size) {
+            r.status = LZ4B200_FRAME_CONTENT_LENGTH;
+            r.err_expected = w.content_size;
+            r.err_actual = r.written;
         }
     }
+    const bool h = p.content && (w.flg & 0x04) && !full;
+    if (h && p.delivered == 0) fw::xxh32_reset(*p.content, 0);
     hash[g] = h;
-    results[f] = r;
+    *p.result = r;
 }
 
-// The content hash of each frame of the group that still needs one, one CTA per frame over its delivered output, carried
-// in states[g] (reset by the resolve step); frame_batch_digest_kernel then compares the digests.
-// frame_out_off and results start at the group's first frame.  (The minimum of one CTA per SM lifts the 40-register
-// limit ptxas otherwise picks here, which spills; it runs at 55 registers, four CTAs per SM.)
-__global__ void __launch_bounds__(256, 1) frame_batch_hash_kernel(const uint8_t *out, const uint64_t *frame_out_off,
-                                                               const uint8_t *hash, lz4b200_xxh32_state *states,
-                                                               const lz4b200_frame_result *results)
+// The content hash of the group's output, one CTA per frame, carried in the frame's state; frame_batch_digest_kernel
+// then compares the digest at the EndMark.  (The minimum of one CTA per SM lifts the 40-register limit ptxas otherwise
+// picks here, which spills.)
+__global__ void __launch_bounds__(256, 1) frame_batch_hash_kernel(const uint8_t *out, const GroupFrame *frames,
+                                                                  const uint8_t *hash)
 {
     __shared__ __align__(16) uint8_t stage[2][kHashChunk + 16];
     const uint32_t g = blockIdx.x;
-    if (hash[g]) content_hash_cta(states + g, out + frame_out_off[g], results[g].written, stage);
+    if (!hash[g]) return;
+    const GroupFrame &p = frames[g];
+    content_hash_cta(p.content, out + p.out_off, p.result->written - p.delivered, stage);
 }
 
-__global__ void __launch_bounds__(128) frame_batch_digest_kernel(uint32_t f0, uint32_t gn, const fw::FrameWalk *walks,
-                                                                 const uint8_t *hash, const lz4b200_xxh32_state *states,
-                                                                 lz4b200_frame_result *results)
+__global__ void __launch_bounds__(128) frame_batch_digest_kernel(const GroupFrame *frames, uint32_t gn,
+                                                                 const uint8_t *hash)
 {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g < gn && hash[g] && fw::xxh32_digest(states[g]) != walks[f0 + g].content_checksum)
-        results[f0 + g].status = LZ4B200_FRAME_CONTENT_CHECKSUM;
+    if (g >= gn || !hash[g]) return;
+    const GroupFrame &p = frames[g];
+    const fw::FrameWalk &w = *p.walk;
+    if (p.last && p.result->status == LZ4B200_OK && w.closed && w.has_checksum &&
+        fw::xxh32_digest(*p.content) != w.content_checksum)
+        p.result->status = LZ4B200_FRAME_CONTENT_CHECKSUM;
 }
 
 }  // namespace lz4b200
@@ -777,21 +811,22 @@ struct lz4b200_ctx {
     DevBuf<uint8_t> d_in, d_out, d_slots, d_flags, d_pick, d_dict;
     DevBuf<uint64_t> d_in_off, d_out_off, d_seg_off, d_expected, d_off_b;
     DevBuf<uint32_t> d_in_len, d_out_cap, d_out_len, d_info, d_seg_size, d_payload_len, d_link_first, d_stored_len, d_done;
-    DevBuf<uint64_t> d_stored_off;
     DevBuf<int32_t> d_status;
     // device-resident frame decoder: walk state, the block descriptors of one walk launch, the first block whose
-    // checksum fails, the running content hash
+    // checksum fails, the running content hash, and the group loop's result
     DevBuf<fw::FrameWalk> d_walk;
     DevBuf<fw::FrameBlockDesc> d_desc;
     DevBuf<uint32_t> d_bad;
     DevBuf<lz4b200_xxh32_state> d_content;
-    // batch frame decoder: per frame the walk, the count and the two block counts; per group the scans, the frames'
-    // descriptor bases, first bad blocks and hash flags; per block its frame, slot bytes and gather lengths
+    DevBuf<lz4b200_frame_result> d_result;
+    // batch frame decoder: per frame the walk, the count and the two block counts; per group the scans and the hash
+    // flags; per block its frame, slot bytes and gather lengths
     DevBuf<fw::FrameWalk> d_fwalk;
     DevBuf<fw::FrameCount> d_fcount;
-    DevBuf<uint32_t> d_fnb, d_fbase, d_fbad, d_bframe, d_bslot, d_glen;
+    DevBuf<uint32_t> d_fnb, d_bframe, d_bslot, d_glen;
     DevBuf<uint64_t> d_fscan, d_gdst;
     DevBuf<uint8_t> d_fhash;
+    DevBuf<GroupFrame> d_gframe;              // the frames of a decode group
     DevBuf<fb::FramePlan> d_fplan;            // batch frame encoder: the host's plan, one entry per frame
 
     bool check(cudaError_t e, const char *what)
@@ -1310,7 +1345,8 @@ void lz4b200_ctx_destroy(lz4b200_ctx *ctx)
     ctx->d_in_len.release(); ctx->d_out_cap.release(); ctx->d_out_len.release(); ctx->d_info.release();
     ctx->d_seg_size.release(); ctx->d_payload_len.release(); ctx->d_status.release();
     ctx->d_gtab16.release();
-    ctx->d_walk.release(); ctx->d_desc.release(); ctx->d_bad.release(); ctx->d_content.release();
+    ctx->d_walk.release(); ctx->d_desc.release(); ctx->d_bad.release(); ctx->d_content.release(); ctx->d_result.release();
+    ctx->d_gframe.release();
 #ifdef LZ4B200_AB_VARIANTS
     ctx->d_ttab16.release(); ctx->d_gtag32.release();
 #endif
@@ -2554,175 +2590,168 @@ lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool d
     return LZ4B200_OK;
 }
 
-// Decodes the blocks a walk recorded, in groups whose device slots fit the context's frame budget (slots are reused
-// from group to group), so a frame of many short blocks costs O(budget) device memory, not #blocks x block size.
-// `in` and `out` are host memory (each group's payload is staged to the device and its output copied back), or with
-// `device` device memory, read and written in place.  When the frame has a content checksum, `content` (host memory,
-// or device memory with `device`) is carried over each group's output.  *written: the bytes delivered.
+// The group pipeline (see GroupFrame) over the gn frames at ctx->d_gframe, whose nb blocks (the nind independent ones
+// first) are described at ctx->d_desc and ctx->d_bframe and whose slots take `slots` bytes: payload read at src, output
+// gathered into out.  Everything is enqueued on s.
+lz4b200_status decode_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *src, uint8_t *out, uint32_t gn, uint32_t nb,
+                            uint32_t nind, uint64_t slots)
+{
+    const uint32_t nlnk = nb - nind, fgrid = (gn + 127) / 128, bgrid = (nb + 127) / 128;
+    GroupFrame *frames = ctx->d_gframe.p;
+    CTX_CUDA(ctx, ctx->d_fhash.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb + 1)); CTX_CUDA(ctx, ctx->d_slots.reserve(slots + 16));
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_pick.reserve(nb)); CTX_CUDA(ctx, ctx->d_link_first.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_stored_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_done.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_bslot.reserve(nb)); CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    if (nb) {
+        frame_batch_args_kernel<<<bgrid, 128, 0, s>>>(frames, ctx->d_desc.p, ctx->d_bframe.p, nb, nind, ctx->d_in_off.p,
+                                                      ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_pick.p,
+                                                      ctx->d_link_first.p, ctx->d_stored_len.p, ctx->d_done.p,
+                                                      ctx->d_bslot.p);
+        scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_bslot.p, ctx->d_out_off.p, nb);
+        CTX_CUDA(ctx, cudaGetLastError());
+        BatchArgs a{src, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
+                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, nind, nullptr};
+        const lz4b200_status st = launch_decompress(ctx, a, s);
+        if (st != LZ4B200_OK) return st;
+        if (nlnk) {
+            // BlockMode::Linked (frame/decompress.rs:196-222): every linked chain of the group in one launch; block b
+            // waits only for blocks [link_first[b], b) of its frame and resolves offsets that reach before it in their
+            // outputs
+            BatchArgs l{src, ctx->d_in_off.p + nind, ctx->d_in_len.p + nind, nullptr, ctx->d_slots.p,
+                        ctx->d_out_off.p + nind, ctx->d_out_cap.p + nind, ctx->d_out_len.p + nind,
+                        ctx->d_status.p + nind, ctx->d_expected.p + nind, nlnk, ctx->d_tickets};
+            l.link_first = ctx->d_link_first.p + nind; l.stored_off = ctx->d_in_off.p + nind;
+            l.stored_len = ctx->d_stored_len.p + nind; l.done = ctx->d_done.p + nind;
+            lz4_decompress_blocks_linked<32><<<std::min<uint32_t>((nlnk + 3) / 4, (uint32_t)ctx->sm_count * 8), 128, 0, s>>>(l);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    frame_resolve_kernel<<<(gn + 3) / 4, 128, 0, s>>>(frames, gn, ctx->d_desc.p, ctx->d_out_len.p, ctx->d_status.p,
+                                               ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_gdst.p, ctx->d_glen.p,
+                                               ctx->d_fhash.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        GatherArgs g{ctx->d_slots.p, src, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_glen.p, ctx->d_glen.p,
+                     ctx->d_pick.p, nullptr, out, ctx->d_gdst.p, nb};
+        gather_segments_kernel<<<std::min<uint32_t>(nb, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    frame_batch_hash_kernel<<<gn, 256, 0, s>>>(out, frames, ctx->d_fhash.p);
+    frame_batch_digest_kernel<<<fgrid, 128, 0, s>>>(frames, gn, ctx->d_fhash.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+// Decodes the blocks a walk `w` recorded through the group pipeline, in groups whose device slots fit the context's
+// frame budget (slots are reused from group to group), so a frame of many short blocks costs O(budget) device memory,
+// not #blocks x block size.  `in` and `out` are host memory (each group's payload is staged to the device and its
+// output copied back), or with `device` device memory, read and written in place.  The frame delivered `delivered`
+// bytes before blocks[0], whose output goes to out[0]; `last`: the blocks end the frame.  `content` carries the
+// frame's content hash: device memory, or with host memory (`device` false) the host hashes each group's output as it
+// lands and the caller compares the digest (one CPU core hashes faster than the GPU's one XXH32 chain).  *r receives the frame's result after the last group decoded (the first that does
+// not return LZ4B200_OK stops the loop), and so does *d_result (device memory) if not null.
 // A linked frame's blocks may continue one decoded earlier (the streaming decoder, device memory only): `window` holds
 // the last `window_len` (<= 64 KiB) bytes of the frame's output before blocks[0], and the linked kernel sees it as a
 // stored block ahead of the group, staged with the group's payload in one buffer.  On FRAME_DECOMPRESSION_ERROR,
 // *failed (if not null) receives the index of the block that failed.
 lz4b200_status decode_frame_blocks(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, uint8_t *out,
                                    size_t cap, const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks,
-                                   lz4b200_xxh32_state *content, size_t *written, int *block_status,
-                                   uint64_t *err_expected, uint64_t *err_actual, const uint8_t *window = nullptr,
+                                   bool last, uint64_t delivered, lz4b200_xxh32_state *content, lz4b200_frame_result *r,
+                                   lz4b200_frame_result *d_result = nullptr, const uint8_t *window = nullptr,
                                    uint32_t window_len = 0, uint32_t *failed = nullptr)
 {
     const uint32_t nb = (uint32_t)blocks.size();
-    const uint64_t bs = w.bs;
-    uint64_t total = 0;
-    *written = 0;
-    if (!nb) return LZ4B200_OK;
+    *r = lz4b200_frame_result{};
+    r->written = delivered;
+    if (!nb && !last) return LZ4B200_OK;                                 // nothing to decode and nothing to decide
     DeviceGuard guard(ctx->device);
-    const bool linked = w.linked && (nb > 1 || window_len > 0);
+    const bool linked = nb && w.linked && (nb > 1 || window_len > 0);
     const uint32_t pre = linked && window_len ? 1 : 0;                   // the window's pseudo-block ahead of the group
-    std::vector<uint64_t> h_in_off, h_slot_off, seg, h_soff;
-    std::vector<uint32_t> h_in_len, h_cap, produced, h_first, h_slen;
-    std::vector<uint8_t> h_pick;
-    std::vector<int32_t> status;
-    std::vector<uint64_t> expected;
-    for (uint32_t g0 = 0; g0 < nb;) {
+    CTX_CUDA(ctx, ctx->d_walk.reserve(1)); CTX_CUDA(ctx, ctx->d_gframe.reserve(1)); CTX_CUDA(ctx, ctx->d_result.reserve(1));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p, &w, sizeof w, cudaMemcpyHostToDevice, s));
+    uint64_t got = 0;                                                     // the bytes delivered from blocks[0] on
+    uint32_t g0 = 0;
+    do {
         // a group: as many blocks as fit the budget (a linked frame is one dependency chain: one group)
         uint32_t g1 = g0;
         uint64_t slot_total = 0;
         while (g1 < nb) {
-            const uint64_t c = fw::block_slot_cap(blocks[g1], bs);
+            const uint64_t c = fw::block_slot_cap(blocks[g1], w.bs);
             const uint64_t in_span = blocks[g1].payload_off + fw::block_len(blocks[g1]) - blocks[g0].payload_off;
             if (!linked && g1 > g0 && fw::group_cut(slot_total, c, in_span, ctx->frame_budget)) break;
             slot_total += fw::slot_bytes(c);
             g1++;
         }
         const uint32_t gn = g1 - g0, gm = gn + pre;                      // the kernel's blocks: [window,] the group
-        const uint64_t in_lo = blocks[g0].payload_off;
-        const uint64_t in_bytes = blocks[g1 - 1].payload_off + fw::block_len(blocks[g1 - 1]) - in_lo;
+        const uint64_t in_lo = gn ? blocks[g0].payload_off : 0;
+        const uint64_t in_bytes = gn ? blocks[g1 - 1].payload_off + fw::block_len(blocks[g1 - 1]) - in_lo : 0;
         const uint64_t shift = pre ? window_len : 0;                       // the payload's place in a staged buffer
-        h_in_off.assign(gm, 0); h_slot_off.assign(gm, 0); h_in_len.assign(gm, 0); h_cap.assign(gm, 0);
-        h_pick.assign(gm, 0); produced.assign(gn, 0); status.assign(gn, 0); expected.assign(gn, 0); seg.assign(gn + 1, 0);
-        if (pre) h_pick[0] = 1;
-        uint64_t so = 0;
-        for (uint32_t k = 0; k < gn; k++) {
-            const fw::FrameBlockDesc &b = blocks[g0 + k];
-            const bool stored = fw::block_stored(b);
-            const uint32_t i = pre + k;
-            h_in_off[i] = b.payload_off - in_lo + shift;
-            h_in_len[i] = stored ? 0 : fw::block_len(b);                 // stored blocks are only gathered
-            h_pick[i] = stored ? 1 : 0;
-            h_slot_off[i] = so;
-            h_cap[i] = (uint32_t)fw::block_slot_cap(b, bs);
-            so += fw::slot_bytes(h_cap[i]);
-        }
-        const uint8_t *src = in + in_lo;                                   // the group's payload on the device
-        if (!device || pre) {
+        GroupFrame p{};
+        const uint8_t *src = in;                                           // the frame's payload on the device
+        if (gn && (!device || pre)) {
             CTX_CUDA(ctx, ctx->d_in.reserve(shift + in_bytes + 16));
-            if (pre) {
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, window, window_len, cudaMemcpyDeviceToDevice, s));
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p + shift, in + in_lo, in_bytes, cudaMemcpyDeviceToDevice, s));
-            } else {
-                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, in + in_lo, in_bytes, cudaMemcpyHostToDevice, s));
-            }
+            if (pre) CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p, window, window_len, cudaMemcpyDeviceToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in.p + shift, in + in_lo, in_bytes,
+                                          device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
             src = ctx->d_in.p;
+            p.in_off = shift - in_lo;                                      // mod 2^64: payload offsets add back to it
         }
-        CTX_CUDA(ctx, ctx->d_slots.reserve(so + 16));
-        CTX_CUDA(ctx, ctx->d_in_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_in_len.reserve(gm));
-        CTX_CUDA(ctx, ctx->d_out_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(gm));
-        CTX_CUDA(ctx, ctx->d_out_len.reserve(gm)); CTX_CUDA(ctx, ctx->d_status.reserve(gm));
-        CTX_CUDA(ctx, ctx->d_expected.reserve(gm));
-        CTX_CUDA(ctx, ctx->d_pick.reserve(gm)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(gn + 1));
-        CTX_CUDA(ctx, ctx->d_payload_len.reserve(gn));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), gm * 8, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, h_in_len.data(), gm * 4, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_off.p, h_slot_off.data(), gm * 8, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_out_cap.p, h_cap.data(), gm * 4, cudaMemcpyHostToDevice, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_pick.p, h_pick.data(), gm, cudaMemcpyHostToDevice, s));
-        BatchArgs a{src, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
-                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, gm, nullptr};
-        lz4b200_status st;
-        if (linked) {
-            // BlockMode::Linked (frame/decompress.rs:196-222): the blocks of a frame form a dependency chain; the
-            // linked kernel resolves offsets that reach before a block in the outputs of its predecessors
-            h_first.assign(gm, 0); h_slen.assign(gm, 0); h_soff.assign(gm, 0);
-            if (pre) h_slen[0] = window_len;
-            for (uint32_t k = 0; k < gn; k++) {
-                h_slen[pre + k] = fw::block_stored(blocks[g0 + k]) ? fw::block_len(blocks[g0 + k]) : 0;
-                h_soff[pre + k] = h_in_off[pre + k];
-            }
-            CTX_CUDA(ctx, ctx->d_link_first.reserve(gm)); CTX_CUDA(ctx, ctx->d_stored_len.reserve(gm));
-            CTX_CUDA(ctx, ctx->d_stored_off.reserve(gm)); CTX_CUDA(ctx, ctx->d_done.reserve(gm));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_link_first.p, h_first.data(), gm * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_len.p, h_slen.data(), gm * 4, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_stored_off.p, h_soff.data(), gm * 8, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_done.p, 0, gm * 4, s));
-            a.link_first = ctx->d_link_first.p; a.stored_off = ctx->d_stored_off.p;
-            a.stored_len = ctx->d_stored_len.p; a.done = ctx->d_done.p;
-            a.tickets = ctx->d_tickets;
-            const uint32_t grid = std::min<uint32_t>((gm + 3) / 4, (uint32_t)ctx->sm_count * 8);
-            lz4_decompress_blocks_linked<32><<<grid, 128, 0, s>>>(a);
-            st = ctx->check(cudaGetLastError(), "linked decode launch") ? LZ4B200_OK : LZ4B200_CUDA_ERROR;
+        uint8_t *dst = out;                                                // the device path gathers in place
+        if (device) {
+            p.out_off = got;
         } else {
-            st = launch_decompress(ctx, a, s);
+            CTX_CUDA(ctx, ctx->d_out.reserve(std::min<uint64_t>(cap - got, slot_total + in_bytes) + 16));
+            dst = ctx->d_out.p;
         }
+        p.out_cap = cap - got;
+        p.delivered = delivered + got;
+        p.walk = ctx->d_walk.p;
+        p.content = device ? content : nullptr;
+        p.result = d_result ? d_result : ctx->d_result.p;
+        p.nblocks = gm;
+        p.bad = fw::kNoBlock;
+        p.window = (uint8_t)pre;
+        p.last = last && g1 == nb;
+        CTX_CUDA(ctx, ctx->d_desc.reserve(gm)); CTX_CUDA(ctx, ctx->d_bframe.reserve(gm));
+        if (pre) {
+            const fw::FrameBlockDesc wd{in_lo - shift, window_len | 0x80000000u, 0};   // stored at the staged buffer's start
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_desc.p, &wd, sizeof wd, cudaMemcpyHostToDevice, s));
+        }
+        if (gn) CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_desc.p + pre, blocks.data() + g0, gn * sizeof(fw::FrameBlockDesc),
+                                              cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bframe.p, 0, gm * sizeof(uint32_t), s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_gframe.p, &p, sizeof p, cudaMemcpyHostToDevice, s));
+        const lz4b200_status st = decode_group(ctx, s, src, dst, 1, gm, linked ? 0 : gm, slot_total);
         if (st != LZ4B200_OK) return st;
-        CTX_CUDA(ctx, cudaMemcpyAsync(produced.data(), ctx->d_out_len.p + pre, gn * 4, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(status.data(), ctx->d_status.p + pre, gn * 4, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaMemcpyAsync(expected.data(), ctx->d_expected.p + pre, gn * 8, cudaMemcpyDeviceToHost, s));
+        uint32_t bad = fw::kNoBlock;
+        CTX_CUDA(ctx, cudaMemcpyAsync(r, p.result, sizeof *r, cudaMemcpyDeviceToHost, s));
+        if (failed) CTX_CUDA(ctx, cudaMemcpyAsync(&bad, &ctx->d_gframe.p->bad, sizeof bad, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaStreamSynchronize(s));
-
-        // first failing block (stream order) wins over anything the walk found later
-        uint32_t good = gn;
-        for (uint32_t k = 0; k < gn; k++) {
-            if (fw::block_stored(blocks[g0 + k])) { produced[k] = fw::block_len(blocks[g0 + k]); status[k] = 0; continue; }
-            if (status[k] != 0) { good = k; break; }
+        const uint64_t n = r->written - p.delivered;
+        if (!device && n) {
+            CTX_CUDA(ctx, cudaMemcpyAsync(out + got, ctx->d_out.p, n, cudaMemcpyDeviceToHost, s));
+            CTX_CUDA(ctx, cudaStreamSynchronize(s));
+            if (w.flg & 0x04) fw::xxh32_update(*content, out + got, n);
         }
-        uint64_t gtotal = 0;
-        for (uint32_t k = 0; k < good; k++) { seg[k] = gtotal; gtotal += produced[k]; }
-        seg[good] = gtotal;
-        if (total + gtotal > cap) { *written = total; return LZ4B200_FRAME_OUTPUT_FULL; }
-        if (gtotal) {
-            uint8_t *dst = out + total;                                    // the device path gathers in place
-            if (!device) {
-                CTX_CUDA(ctx, ctx->d_out.reserve(gtotal + 16));
-                dst = ctx->d_out.p;
-            }
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_seg_off.p, seg.data(), (good + 1) * 8, cudaMemcpyHostToDevice, s));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_payload_len.p, produced.data(), good * 4, cudaMemcpyHostToDevice, s));
-            GatherArgs g{ctx->d_slots.p, src, ctx->d_out_off.p + pre, ctx->d_in_off.p + pre, ctx->d_payload_len.p,
-                         ctx->d_payload_len.p, ctx->d_pick.p + pre, nullptr, dst, ctx->d_seg_off.p, good};
-            gather_segments_kernel<<<std::min<uint32_t>(good, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
-            CTX_CUDA(ctx, cudaGetLastError());
-            if (device) {
-                if (w.has_checksum) {
-                    content_hash_kernel<<<1, 256, 0, s>>>(content, out + total, gtotal);
-                    CTX_CUDA(ctx, cudaGetLastError());
-                }
-            } else {
-                CTX_CUDA(ctx, cudaMemcpyAsync(out + total, ctx->d_out.p, gtotal, cudaMemcpyDeviceToHost, s));
-                CTX_CUDA(ctx, cudaStreamSynchronize(s));
-                if (w.has_checksum) fw::xxh32_update(*content, out + total, gtotal);
-            }
-        }
-        total += gtotal;
-        *written = total;
-        if (good < gn) {
-            if (block_status) *block_status = status[good];
-            if (status[good] == LZ4B200_DEC_OUTPUT_TOO_SMALL) {
-                if (err_expected) *err_expected = expected[good];
-                if (err_actual) *err_actual = h_cap[pre + good];
-            }
-            if (failed) *failed = g0 + good;
-            return LZ4B200_FRAME_DECOMPRESSION_ERROR;
-        }
+        got += n;
+        if (failed && r->status == LZ4B200_FRAME_DECOMPRESSION_ERROR) *failed = g0 + bad;
         g0 = g1;
-    }
+    } while (r->status == LZ4B200_OK && g0 < nb);
     return LZ4B200_OK;
 }
 
-// One frame, FrameDecoder::read_to_end (frame/decompress.rs:109-342): walk, block checksums, decode, then content size
-// and checksum at the EndMark.  `in` and `out` are host memory, or device memory with `device`; both paths run the same
-// walk and the same group loop, so they return the same result for the same bytes.
+// One frame, FrameDecoder::read_to_end (frame/decompress.rs:109-342): walk, block checksums, then the group loop, whose
+// last group decides the content size and checksum at the EndMark.  `in` and `out` are host memory, or device memory
+// with `device`; both paths run the same walk and the same group loop, so they return the same result for the same
+// bytes.  *d_result (device memory), if not null, also receives the result.
 lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, size_t n,
                                           uint8_t *out, size_t cap, size_t *consumed, size_t *written, int *block_status,
-                                          uint64_t *err_expected, uint64_t *err_actual)
+                                          uint64_t *err_expected, uint64_t *err_actual,
+                                          lz4b200_frame_result *d_result = nullptr)
 {
     *written = 0; *consumed = 0;
     if (block_status) *block_status = 0;
@@ -2745,108 +2774,47 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
         blocks.resize(bad);
     }
     *consumed = w.ip;
-
-    lz4b200_xxh32_state content;
-    fw::xxh32_reset(content, 0);
-    lz4b200_xxh32_state *cs = &content;
-    if (device && w.has_checksum && !blocks.empty()) {
-        CTX_CUDA(ctx, ctx->d_content.reserve(1));
-        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_content.p, &content, sizeof content, cudaMemcpyHostToDevice, s));
-        cs = ctx->d_content.p;
-    }
-    size_t total = 0;
-    const lz4b200_status st = decode_frame_blocks(ctx, s, device, in, out, cap, w, blocks, cs, &total, block_status,
-                                                  err_expected, err_actual);
-    *written = total;
+    lz4b200_xxh32_state host_content;
+    fw::xxh32_reset(host_content, 0);
+    if (device) CTX_CUDA(ctx, ctx->d_content.reserve(1));
+    lz4b200_frame_result r;
+    const lz4b200_status st = decode_frame_blocks(ctx, s, device, in, out, cap, w, blocks, true, 0,
+                                                  device ? ctx->d_content.p : &host_content, &r, d_result);
+    *written = r.written;
     if (st != LZ4B200_OK) return st;
-    if (w.status != LZ4B200_OK) return (lz4b200_status)w.status;
-
-    // ---- content size / checksum at the EndMark (decompress.rs:312-331) ---------------------------------------------------
-    if (w.closed) {
-        if (w.has_size && total != w.content_size) {
-            if (err_expected) *err_expected = w.content_size;
-            if (err_actual) *err_actual = total;
-            return LZ4B200_FRAME_CONTENT_LENGTH;
-        }
-        if (w.has_checksum) {
-            if (cs != &content) {
-                CTX_CUDA(ctx, cudaMemcpyAsync(&content, cs, sizeof content, cudaMemcpyDeviceToHost, s));
-                CTX_CUDA(ctx, cudaStreamSynchronize(s));
-            }
-            if (fw::xxh32_digest(content) != w.content_checksum) return LZ4B200_FRAME_CONTENT_CHECKSUM;
-        }
-    }
-    return LZ4B200_OK;
+    if (!device && r.status == LZ4B200_OK && w.closed && w.has_checksum &&
+        fw::xxh32_digest(host_content) != w.content_checksum)
+        r.status = LZ4B200_FRAME_CONTENT_CHECKSUM;           // the digest kernel's rule, for the host's hash
+    if (block_status) *block_status = r.block_status;
+    if (err_expected) *err_expected = r.err_expected;
+    if (err_actual) *err_actual = r.err_actual;
+    return (lz4b200_status)r.status;
 }
 
 // A group of the batch: frames [f0, f0 + gn), each of which the group loop decodes as one group, with nind blocks of
-// independent frames and nlnk of linked frames whose slots take `slots` bytes.  Record walk, block checksums, one
-// decode launch per class, resolve, one gather and the per-frame content hash, all enqueued on s.
+// independent frames and nlnk of linked frames whose slots take `slots` bytes.  Record walk and block checksums, then
+// the group pipeline, all enqueued on s.
 lz4b200_status decode_frame_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off,
                                   const uint64_t *d_frame_len, uint8_t *d_out, const uint64_t *d_out_off,
                                   const uint64_t *d_out_cap, lz4b200_frame_result *d_results, uint32_t nframes,
                                   uint32_t f0, uint32_t gn, uint32_t nind, uint32_t nlnk, uint64_t slots)
 {
     const uint32_t nb = nind + nlnk;
-    const uint32_t fgrid = (gn + 127) / 128, bgrid = (nb + 127) / 128;
-    CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_fbase.reserve(gn));
-    CTX_CUDA(ctx, ctx->d_fbad.reserve(gn)); CTX_CUDA(ctx, ctx->d_fhash.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_gframe.reserve(gn));
     CTX_CUDA(ctx, ctx->d_content.reserve(gn));
-    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb)); CTX_CUDA(ctx, ctx->d_bslot.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb + 1)); CTX_CUDA(ctx, ctx->d_slots.reserve(slots + 16));
-    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_pick.reserve(nb)); CTX_CUDA(ctx, ctx->d_link_first.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_stored_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_done.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb));
     uint64_t *scan_ind = ctx->d_fscan.p, *scan_lnk = ctx->d_fscan.p + gn + 1;
 
     scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + f0, scan_ind, gn);
     scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + nframes + f0, scan_lnk, gn);
-    frame_record_kernel<<<fgrid, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, f0, gn, ctx->d_fwalk.p, ctx->d_fcount.p,
-                                              scan_ind, scan_lnk, ctx->d_desc.p, ctx->d_fbase.p, ctx->d_bframe.p,
-                                              ctx->d_bslot.p, ctx->d_fbad.p);
+    frame_record_kernel<<<(gn + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, f0, gn,
+                                                         ctx->d_fwalk.p, ctx->d_fcount.p, scan_ind, scan_lnk,
+                                                         ctx->d_desc.p, ctx->d_bframe.p, ctx->d_content.p, d_results,
+                                                         ctx->d_gframe.p);
+    if (nb) frame_batch_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, nb,
+                                                                        ctx->d_gframe.p);
     CTX_CUDA(ctx, cudaGetLastError());
-    if (nb) {
-        frame_batch_checksum_kernel<<<bgrid, 128, 0, s>>>(d_in, d_frame_off, f0, ctx->d_fwalk.p, ctx->d_desc.p,
-                                                          ctx->d_fbase.p, ctx->d_bframe.p, nb, ctx->d_fbad.p);
-        scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_bslot.p, ctx->d_out_off.p, nb);
-        frame_batch_args_kernel<<<bgrid, 128, 0, s>>>(d_frame_off, f0, ctx->d_fwalk.p, ctx->d_desc.p, ctx->d_fbase.p,
-                                                      ctx->d_bframe.p, ctx->d_fbad.p, nb, nind, ctx->d_in_off.p,
-                                                      ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_pick.p,
-                                                      ctx->d_link_first.p, ctx->d_stored_len.p, ctx->d_done.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, ctx->d_slots.p, ctx->d_out_off.p,
-                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p, nind, nullptr};
-        const lz4b200_status st = launch_decompress(ctx, a, s);
-        if (st != LZ4B200_OK) return st;
-        if (nlnk) {
-            // every linked chain of the group in one launch: block b waits only for blocks [link_first[b], b) of its frame
-            BatchArgs l{d_in, ctx->d_in_off.p + nind, ctx->d_in_len.p + nind, nullptr, ctx->d_slots.p,
-                        ctx->d_out_off.p + nind, ctx->d_out_cap.p + nind, ctx->d_out_len.p + nind,
-                        ctx->d_status.p + nind, ctx->d_expected.p + nind, nlnk, ctx->d_tickets};
-            l.link_first = ctx->d_link_first.p + nind; l.stored_off = ctx->d_in_off.p + nind;
-            l.stored_len = ctx->d_stored_len.p + nind; l.done = ctx->d_done.p + nind;
-            lz4_decompress_blocks_linked<32><<<std::min<uint32_t>((nlnk + 3) / 4, (uint32_t)ctx->sm_count * 8), 128, 0, s>>>(l);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
-    }
-    frame_resolve_kernel<<<fgrid, 128, 0, s>>>(f0, gn, ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_desc.p, ctx->d_fbase.p,
-                                               ctx->d_fbad.p, ctx->d_out_len.p, ctx->d_status.p, ctx->d_expected.p,
-                                               ctx->d_out_cap.p, d_out_off, d_out_cap, ctx->d_gdst.p, ctx->d_glen.p,
-                                               ctx->d_fhash.p, ctx->d_content.p, d_results);
-    CTX_CUDA(ctx, cudaGetLastError());
-    if (nb) {
-        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_glen.p, ctx->d_glen.p,
-                     ctx->d_pick.p, nullptr, d_out, ctx->d_gdst.p, nb};
-        gather_segments_kernel<<<std::min<uint32_t>(nb, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
-        CTX_CUDA(ctx, cudaGetLastError());
-    }
-    frame_batch_hash_kernel<<<gn, 256, 0, s>>>(d_out, d_out_off + f0, ctx->d_fhash.p, ctx->d_content.p, d_results + f0);
-    frame_batch_digest_kernel<<<fgrid, 128, 0, s>>>(f0, gn, ctx->d_fwalk.p, ctx->d_fhash.p, ctx->d_content.p, d_results);
-    CTX_CUDA(ctx, cudaGetLastError());
-    return LZ4B200_OK;
+    return decode_group(ctx, s, d_in, d_out, gn, nb, nind, slots);
 }
 
 }  // namespace
@@ -2883,7 +2851,7 @@ lz4b200_status lz4b200_frame_decompress_next(lz4b200_ctx *ctx, const uint8_t *in
 }
 
 // One frame from device memory into device memory: walk, block checksums, decode and content checksum on the GPU; only
-// block descriptors, per-group statuses and the 48-byte hash state cross PCIe.
+// the walk, block descriptors and one result per group cross PCIe.
 lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint8_t *d_out,
                                                     size_t cap, size_t *consumed, size_t *written, int *block_status,
                                                     uint64_t *err_expected, uint64_t *err_actual, void *stream)
@@ -2951,26 +2919,20 @@ lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx, const uin
     if (st != LZ4B200_OK) return st;
     if (!solo.empty()) {
         // frames the group loop splits (at least one budget of slots) or with more blocks than a group holds: the
-        // one-frame device call, which runs the group loop over them
+        // one-frame device call, which runs the group loop over them and writes their results on the device (every such
+        // frame has blocks, so the loop runs)
         std::vector<uint64_t> off(n), len(n), ooff(n), ocap(n);
         CTX_CUDA(ctx, cudaMemcpyAsync(off.data(), d_frame_off, n * 8ull, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaMemcpyAsync(len.data(), d_frame_len, n * 8ull, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaMemcpyAsync(ooff.data(), d_out_off, n * 8ull, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaMemcpyAsync(ocap.data(), d_out_cap, n * 8ull, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaStreamSynchronize(s));
-        std::vector<lz4b200_frame_result> res(solo.size());
-        for (size_t i = 0; i < solo.size(); i++) {
-            const uint32_t f = solo[i];
-            lz4b200_frame_result &r = res[i];
+        for (const uint32_t f : solo) {
             size_t consumed = 0, written = 0;
-            int bs = 0;
-            r.status = frame_decompress_next_impl(ctx, s, true, d_in + off[f], len[f], d_out + ooff[f], ocap[f],
-                                                  &consumed, &written, &bs, &r.err_expected, &r.err_actual);
-            if (r.status == LZ4B200_CUDA_ERROR) return LZ4B200_CUDA_ERROR;
-            r.consumed = consumed; r.written = written; r.block_status = bs;
-            CTX_CUDA(ctx, cudaMemcpyAsync(d_results + f, &r, sizeof r, cudaMemcpyHostToDevice, s));
+            if (frame_decompress_next_impl(ctx, s, true, d_in + off[f], len[f], d_out + ooff[f], ocap[f], &consumed,
+                                           &written, nullptr, nullptr, nullptr, d_results + f) == LZ4B200_CUDA_ERROR)
+                return LZ4B200_CUDA_ERROR;
         }
-        CTX_CUDA(ctx, cudaStreamSynchronize(s));
     }
     CTX_CUDA(ctx, cudaStreamSynchronize(s));
     return LZ4B200_OK;
@@ -3024,10 +2986,11 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_in); add(ctx->d_out); add(ctx->d_slots); add(ctx->d_flags); add(ctx->d_pick); add(ctx->d_dict);
     add(ctx->d_in_off); add(ctx->d_out_off); add(ctx->d_seg_off); add(ctx->d_expected); add(ctx->d_off_b);
     add(ctx->d_in_len); add(ctx->d_out_cap); add(ctx->d_out_len); add(ctx->d_info); add(ctx->d_seg_size);
-    add(ctx->d_payload_len); add(ctx->d_link_first); add(ctx->d_stored_len); add(ctx->d_done); add(ctx->d_stored_off);
-    add(ctx->d_status); add(ctx->d_walk); add(ctx->d_desc); add(ctx->d_bad); add(ctx->d_content);
-    add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_fbase); add(ctx->d_fbad); add(ctx->d_bframe);
+    add(ctx->d_payload_len); add(ctx->d_link_first); add(ctx->d_stored_len); add(ctx->d_done);
+    add(ctx->d_status); add(ctx->d_walk); add(ctx->d_desc); add(ctx->d_bad); add(ctx->d_content); add(ctx->d_result);
+    add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_bframe);
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
+    add(ctx->d_gframe);
     if (const Pipeline *p = static_cast<const Pipeline *>(ctx->pipe)) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
         if (p->d_tickets) b += kMaxLanes * 8 * sizeof(uint32_t);
@@ -3131,52 +3094,29 @@ lz4b200_status decoder_step(lz4b200_frame_decoder *dec, cudaStream_t s, const ui
         wn.content_checksum = 0;
         need = 0;
     }
-    if (w0.stage == fw::kWalkHeader) {
-        lz4b200_xxh32_state c;
-        fw::xxh32_reset(c, 0);
-        CTX_CUDA(ctx, cudaMemcpyAsync(dec->d_content.p, &c, sizeof c, cudaMemcpyHostToDevice, s));
-    }
-
     blocks.resize(t);
-    fw::FrameWalk wd = wn;
-    wd.has_checksum = (wn.flg & 0x04) != 0;                       // hashed as groups land: the EndMark may come later
-    size_t got = 0;
-    int bstat = 0;
-    uint64_t e1 = 0, e2 = 0;
+    lz4b200_frame_result r;
     uint32_t failed = fw::kNoBlock;
-    const lz4b200_status st = decode_frame_blocks(ctx, s, true, d_in, d_out, out_cap, wd, blocks, dec->d_content.p, &got,
-                                                  &bstat, &e1, &e2, dec->d_win.p + (size_t)dec->win * kWindowBytes,
-                                                  dec->win_len, &failed);
-    if (st != LZ4B200_OK && st != LZ4B200_FRAME_DECOMPRESSION_ERROR) return st;
-    dec->written += got;
+    const lz4b200_status st = decode_frame_blocks(ctx, s, true, d_in, d_out, out_cap, wn, blocks,
+                                                  wn.stage == fw::kWalkDone, dec->written, dec->d_content.p, &r, nullptr,
+                                                  dec->d_win.p + (size_t)dec->win * kWindowBytes, dec->win_len, &failed);
+    if (st != LZ4B200_OK) return st;
+    if (r.status == LZ4B200_FRAME_OUTPUT_FULL) return LZ4B200_FRAME_OUTPUT_FULL;
+    const uint64_t got = r.written - dec->written;
+    dec->written = r.written;
     step.written = got;
-    if (st == LZ4B200_FRAME_DECOMPRESSION_ERROR) {
+    if (r.status == LZ4B200_FRAME_DECOMPRESSION_ERROR) {
         // the reference's reader stands after the failing block and its checksum
         const fw::FrameBlockDesc &b = blocks[failed];
         step.consumed = b.payload_off + fw::block_len(b) + ((wn.flg & 0x10) ? 4 : 0);
-        step.result.block_status = bstat;
-        step.result.err_expected = e1;
-        step.result.err_actual = e2;
-        decoder_finish(dec, step, st, at + step.consumed);
+        step.result = r;
+        decoder_finish(dec, step, LZ4B200_FRAME_DECOMPRESSION_ERROR, at + step.consumed);
         return LZ4B200_OK;
     }
     step.consumed = wn.ip - at;
     if (wn.stage == fw::kWalkDone) {
-        // content size and checksum at the EndMark (decompress.rs:312-331)
-        lz4b200_status fs = (lz4b200_status)wn.status;
-        if (fs == LZ4B200_OK && wn.closed) {
-            if (wn.has_size && dec->written != wn.content_size) {
-                fs = LZ4B200_FRAME_CONTENT_LENGTH;
-                step.result.err_expected = wn.content_size;
-                step.result.err_actual = dec->written;
-            } else if (wn.has_checksum) {
-                lz4b200_xxh32_state c;
-                CTX_CUDA(ctx, cudaMemcpyAsync(&c, dec->d_content.p, sizeof c, cudaMemcpyDeviceToHost, s));
-                CTX_CUDA(ctx, cudaStreamSynchronize(s));
-                if (fw::xxh32_digest(c) != wn.content_checksum) fs = LZ4B200_FRAME_CONTENT_CHECKSUM;
-            }
-        }
-        decoder_finish(dec, step, fs, wn.ip);
+        step.result = r;
+        decoder_finish(dec, step, (lz4b200_status)r.status, wn.ip);
         return LZ4B200_OK;
     }
     if (wn.linked && got) {
