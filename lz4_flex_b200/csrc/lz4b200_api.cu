@@ -10,7 +10,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "lz4b200_frame_batch.cuh"
@@ -740,20 +742,64 @@ int auto_block_size_id(size_t first_write_len)
     return 4;
 }
 
+// Device memory, freed with its owner on the owner's device.  reserve() grows with slack; resize() holds exactly n.
 template <typename T> struct DevBuf {
     T *p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+    cudaError_t reserve(size_t n) { return n <= cap ? cudaSuccess : resize(n + n / 8 + 256); }
+    cudaError_t resize(size_t n)
+    {
+        if (p) cudaFree(p);
+        p = nullptr; cap = 0;
+        cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&p), n * sizeof(T));
+        if (e == cudaSuccess) cap = n; else p = nullptr;
+        return e;
+    }
+};
+
+template <typename T> struct PinnedBuf {
+    T *p = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf &) = delete;
+    PinnedBuf &operator=(const PinnedBuf &) = delete;
+    ~PinnedBuf() { if (p) cudaFreeHost(p); }
     cudaError_t reserve(size_t n)
     {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
+        if (p) cudaFreeHost(p);
         p = nullptr; cap = 0;
-        size_t want = n + n / 8 + 256;
-        cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&p), want * sizeof(T));
-        if (e == cudaSuccess) cap = want;
+        cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&p), (n + n / 4 + 64) * sizeof(T), cudaHostAllocDefault);
+        if (e == cudaSuccess) cap = n + n / 4 + 64; else p = nullptr;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+};
+
+constexpr int kMaxLanes = 8;
+
+struct Lane {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t sizes_ready = nullptr;
+    DevBuf<uint8_t> in, slots, out;
+    ~Lane()
+    {
+        if (stream) cudaStreamDestroy(stream);
+        if (sizes_ready) cudaEventDestroy(sizes_ready);
+    }
+};
+
+struct Pipeline {
+    Lane lane[kMaxLanes];
+    cudaEvent_t desc_ready = nullptr;
+    DevBuf<uint32_t> d_tickets;               // kMaxLanes x 8 counters
+    PinnedBuf<uint64_t> h_seg;
+    PinnedBuf<int32_t> h_status;
+    bool ready = false;
+    ~Pipeline() { if (desc_ready) cudaEventDestroy(desc_ready); }
 };
 
 }  // namespace
@@ -761,14 +807,12 @@ template <typename T> struct DevBuf {
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
-static void pipeline_destroy(void *p);
-
 struct lz4b200_ctx {
-    void *pipe = nullptr;                     // host-batch pipeline state (streams, pinned staging), created on demand
+    std::unique_ptr<Pipeline> pipe;           // host-batch pipeline state (streams, pinned staging), created on demand
     int device = 0;
     int sm_count = 0;
     cudaStream_t stream = nullptr;
-    uint32_t *d_tickets = nullptr;            // 3 x {next, retired}
+    DevBuf<uint32_t> d_tickets;               // 3 x {next, retired}
     int dec_ctas_per_sm = 0;
     int enc16s_ctas_per_sm = 0, enc32s_ctas_per_sm = 0;   // split (matcher+emitter) encoder
     int enc_gtab_ctas_per_sm = 0;             // global-table encoder (must reach ENC_GTAB_CTAS)
@@ -834,6 +878,15 @@ struct lz4b200_ctx {
         if (e == cudaSuccess) return true;
         last_error = std::string(what) + ": " + cudaGetErrorString(e);
         return false;
+    }
+
+    __attribute__((visibility("hidden"))) ~lz4b200_ctx()     // not part of the library's exports
+    {
+        if (stream) cudaStreamSynchronize(stream);
+        if (pipe)
+            for (const Lane &l : pipe->lane)
+                if (l.stream) cudaStreamSynchronize(l.stream);
+        if (stream) cudaStreamDestroy(stream);
     }
 };
 
@@ -951,7 +1004,7 @@ lz4b200_status launch_decompress(lz4b200_ctx *ctx, const BatchArgs &args, cudaSt
 {
     if (args.nblocks == 0) return LZ4B200_OK;
     BatchArgs a = args;
-    a.tickets = tickets ? tickets : ctx->d_tickets;
+    a.tickets = tickets ? tickets : ctx->d_tickets.p;
 #ifdef LZ4B200_AB_VARIANTS
     if (!a.dict_len && a.nblocks >= ctx->dec_thread_min) {
         const uint32_t threads = std::min(a.nblocks, ctx->dec_thread_max);
@@ -974,7 +1027,7 @@ lz4b200_status launch_decompress(lz4b200_ctx *ctx, const BatchArgs &args, cudaSt
 // doubles as the region selector.
 static size_t table_slot(const lz4b200_ctx *ctx, const uint32_t *tickets)
 {
-    return tickets == ctx->d_tickets ? 0 : 1 + ((size_t)(tickets - ctx->pipe_tickets) / 8u) % 8u;
+    return tickets == ctx->d_tickets.p ? 0 : 1 + ((size_t)(tickets - ctx->pipe_tickets) / 8u) % 8u;
 }
 
 #ifdef LZ4B200_AB_VARIANTS
@@ -1057,7 +1110,7 @@ static bool launch_compress_variant(lz4b200_ctx *ctx, const BatchArgs &a, uint32
 lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t max_in_len, cudaStream_t s,
                                uint32_t *tickets = nullptr)
 {
-    if (!tickets) tickets = ctx->d_tickets;
+    if (!tickets) tickets = ctx->d_tickets.p;
     if (args.nblocks == 0) return LZ4B200_OK;
     const BatchArgs &a = args;
 #ifdef LZ4B200_AB_VARIANTS
@@ -1222,8 +1275,8 @@ lz4b200_status lz4b200_ctx_create(int device, lz4b200_ctx **out)
     DeviceGuard guard(device);
     bool ok = ctx->check(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device), "sm count") &&
               ctx->check(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking), "stream") &&
-              ctx->check(cudaMalloc(reinterpret_cast<void **>(&ctx->d_tickets), 8 * sizeof(uint32_t)), "tickets") &&
-              ctx->check(cudaMemset(ctx->d_tickets, 0, 8 * sizeof(uint32_t)), "tickets memset");
+              ctx->check(ctx->d_tickets.resize(8), "tickets") &&
+              ctx->check(cudaMemset(ctx->d_tickets.p, 0, 8 * sizeof(uint32_t)), "tickets memset");
     if (ok) {
         ok = ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->dec_ctas_per_sm, lz4_decompress_blocks<8, 0, false>,
                                                                       kDecWarpsPerCta * 32, 0), "occupancy dec") &&
@@ -1336,20 +1389,6 @@ void lz4b200_ctx_destroy(lz4b200_ctx *ctx)
 {
     if (!ctx) return;
     DeviceGuard guard(ctx->device);
-    if (ctx->stream) { cudaStreamSynchronize(ctx->stream); cudaStreamDestroy(ctx->stream); }
-    if (ctx->d_tickets) cudaFree(ctx->d_tickets);
-    pipeline_destroy(ctx->pipe);
-    ctx->d_in.release(); ctx->d_out.release(); ctx->d_slots.release(); ctx->d_flags.release(); ctx->d_pick.release();
-    ctx->d_in_off.release(); ctx->d_out_off.release(); ctx->d_seg_off.release(); ctx->d_expected.release();
-    ctx->d_off_b.release();
-    ctx->d_in_len.release(); ctx->d_out_cap.release(); ctx->d_out_len.release(); ctx->d_info.release();
-    ctx->d_seg_size.release(); ctx->d_payload_len.release(); ctx->d_status.release();
-    ctx->d_gtab16.release();
-    ctx->d_walk.release(); ctx->d_desc.release(); ctx->d_bad.release(); ctx->d_content.release(); ctx->d_result.release();
-    ctx->d_gframe.release();
-#ifdef LZ4B200_AB_VARIANTS
-    ctx->d_ttab16.release(); ctx->d_gtag32.release();
-#endif
     delete ctx;
 }
 
@@ -1602,7 +1641,6 @@ lz4b200_status lz4b200_decompress_size_prepended_batch_device_with_dict(lz4b200_
 
 namespace {
 
-constexpr int kMaxLanes = 8;
 // Lanes in flight.  A compress chunk occupies its lane for H2D + kernel (at least one block's serial chain, several ms)
 // + the size read-back + D2H, so a few lanes cap the call whatever the kernel does; eight lanes leave the kernel / PCIe as
 // the bound.  LZ4B200_LANES overrides.
@@ -1625,76 +1663,35 @@ uint64_t env_mib(const char *name, uint64_t dflt)         // tuning aid: chunk s
     return m > 0 ? (uint64_t)m << 20 : dflt;
 }
 
-struct Lane {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t sizes_ready = nullptr;
-    DevBuf<uint8_t> in, slots, out;
-};
-
-struct Pipeline {
-    Lane lane[kMaxLanes];
-    cudaEvent_t desc_ready = nullptr;
-    uint32_t *d_tickets = nullptr;           // kMaxLanes x 8 counters
-    uint64_t *h_seg = nullptr; size_t h_seg_cap = 0;       // pinned
-    int32_t *h_status = nullptr; size_t h_status_cap = 0;  // pinned
-    bool ready = false;
-};
-
 lz4b200_status pipeline_init(lz4b200_ctx *ctx, Pipeline &p)
 {
     if (p.ready) return LZ4B200_OK;
-    for (int i = 0; i < kMaxLanes; i++) {
-        // LZ4B200_STREAM_PRIORITY=high: this context's kernels get the SM slots first when another context (e.g. a
-        // compress pipeline running next to a decompress pipeline) keeps the GPU full
-        int lo = 0, hi = 0;
-        cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        const int prio = ctx->high_priority ? hi : 0;
-        CTX_CUDA(ctx, cudaStreamCreateWithPriority(&p.lane[i].stream, cudaStreamNonBlocking, prio));
-        CTX_CUDA(ctx, cudaEventCreateWithFlags(&p.lane[i].sizes_ready, cudaEventDisableTiming));
+    // LZ4B200_STREAM_PRIORITY=high: this context's kernels get the SM slots first when another context (e.g. a
+    // compress pipeline running next to a decompress pipeline) keeps the GPU full
+    int lo = 0, hi = 0;
+    cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    const int prio = ctx->high_priority ? hi : 0;
+    for (Lane &l : p.lane) {
+        if (!l.stream) CTX_CUDA(ctx, cudaStreamCreateWithPriority(&l.stream, cudaStreamNonBlocking, prio));
+        if (!l.sizes_ready) CTX_CUDA(ctx, cudaEventCreateWithFlags(&l.sizes_ready, cudaEventDisableTiming));
     }
-    CTX_CUDA(ctx, cudaEventCreateWithFlags(&p.desc_ready, cudaEventDisableTiming));
-    CTX_CUDA(ctx, cudaMalloc(reinterpret_cast<void **>(&p.d_tickets), kMaxLanes * 8 * sizeof(uint32_t)));
-    CTX_CUDA(ctx, cudaMemset(p.d_tickets, 0, kMaxLanes * 8 * sizeof(uint32_t)));
-    ctx->pipe_tickets = p.d_tickets;
+    if (!p.desc_ready) CTX_CUDA(ctx, cudaEventCreateWithFlags(&p.desc_ready, cudaEventDisableTiming));
+    if (!p.d_tickets.p) CTX_CUDA(ctx, p.d_tickets.resize(kMaxLanes * 8));
+    CTX_CUDA(ctx, cudaMemset(p.d_tickets.p, 0, kMaxLanes * 8 * sizeof(uint32_t)));
+    ctx->pipe_tickets = p.d_tickets.p;
     p.ready = true;
     return LZ4B200_OK;
 }
 
-template <typename T> cudaError_t pinned_reserve(T *&ptr, size_t &cap, size_t n)
+Pipeline &ctx_pipeline(lz4b200_ctx *ctx)
 {
-    if (n <= cap) return cudaSuccess;
-    if (ptr) cudaFreeHost(ptr);
-    ptr = nullptr; cap = 0;
-    cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&ptr), (n + n / 4 + 64) * sizeof(T), cudaHostAllocDefault);
-    if (e == cudaSuccess) cap = n + n / 4 + 64;
-    return e;
+    if (!ctx->pipe) ctx->pipe = std::make_unique<Pipeline>();
+    return *ctx->pipe;
 }
 
 struct Chunk { uint32_t b0, b1; uint64_t in_lo, in_hi, a, b; };   // a/b: slot bytes (compress) or out_lo/out_hi (decompress)
 
 }  // namespace
-
-static Pipeline &ctx_pipeline(lz4b200_ctx *ctx)
-{
-    if (!ctx->pipe) ctx->pipe = new Pipeline();
-    return *static_cast<Pipeline *>(ctx->pipe);
-}
-
-static void pipeline_destroy(void *vp)
-{
-    Pipeline *p = static_cast<Pipeline *>(vp);
-    if (!p) return;
-    for (int i = 0; i < kMaxLanes; i++) {
-        if (p->lane[i].stream) { cudaStreamSynchronize(p->lane[i].stream); cudaStreamDestroy(p->lane[i].stream); }
-        if (p->lane[i].sizes_ready) cudaEventDestroy(p->lane[i].sizes_ready);
-        p->lane[i].in.release(); p->lane[i].slots.release(); p->lane[i].out.release();
-    }
-    if (p->desc_ready) cudaEventDestroy(p->desc_ready);
-    if (p->d_tickets) cudaFree(p->d_tickets);
-    if (p->h_seg) cudaFreeHost(p->h_seg);
-    if (p->h_status) cudaFreeHost(p->h_status);
-    delete p;
-}
 
 static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *in, const uint64_t *in_off,
                                                const uint32_t *in_len, const uint8_t *flags, const uint8_t *dict,
@@ -1746,8 +1743,8 @@ static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *
     CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
     CTX_CUDA(ctx, ctx->d_seg_off.reserve(nb + nch));
     if (flags) CTX_CUDA(ctx, ctx->d_flags.reserve(nb));
-    CTX_CUDA(ctx, pinned_reserve(pl.h_seg, pl.h_seg_cap, (size_t)nb + nch));
-    CTX_CUDA(ctx, pinned_reserve(pl.h_status, pl.h_status_cap, nb));
+    CTX_CUDA(ctx, pl.h_seg.reserve((size_t)nb + nch));
+    CTX_CUDA(ctx, pl.h_status.reserve(nb));
 
     cudaStream_t s0 = pl.lane[0].stream;
     CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), nb * 8, cudaMemcpyHostToDevice, s0));
@@ -1775,11 +1772,11 @@ static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *
                     ln.slots.p, ctx->d_out_off.p + c.b0, ctx->d_out_cap.p + c.b0, ctx->d_out_len.p + c.b0,
                     ctx->d_status.p + c.b0, nullptr, n, nullptr};
         if (dict_len) { a.dict = ctx->d_dict.p; a.dict_len = (uint32_t)dict_len; }
-        lz4b200_status r = launch_compress(ctx, a, max_len, ln.stream, pl.d_tickets + 8 * (ci % kLanes));
+        lz4b200_status r = launch_compress(ctx, a, max_len, ln.stream, pl.d_tickets.p + 8 * (ci % kLanes));
         if (r != LZ4B200_OK) return r;
         scan_sizes_kernel<<<1, 1024, 0, ln.stream>>>(ctx->d_out_len.p + c.b0, ctx->d_seg_off.p + c.b0 + ci, n);
         CTX_CUDA(ctx, cudaGetLastError());
-        CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_seg + c.b0 + ci, ctx->d_seg_off.p + c.b0 + ci, (n + 1) * 8,
+        CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_seg.p + c.b0 + ci, ctx->d_seg_off.p + c.b0 + ci, (n + 1) * 8,
                                       cudaMemcpyDeviceToHost, ln.stream));
         CTX_CUDA(ctx, cudaEventRecord(ln.sizes_ready, ln.stream));
         return LZ4B200_OK;
@@ -1796,7 +1793,7 @@ static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *
         Lane &ln = pl.lane[ci % kLanes];
         const uint32_t n = c.b1 - c.b0;
         CTX_CUDA(ctx, cudaEventSynchronize(ln.sizes_ready));
-        const uint64_t *seg = pl.h_seg + c.b0 + ci;
+        const uint64_t *seg = pl.h_seg.p + c.b0 + ci;
         const uint64_t total = seg[n];
         for (uint32_t k = 0; k < n; k++) {
             out_off[c.b0 + k] = out_base + seg[k];
@@ -1819,9 +1816,9 @@ static lz4b200_status compress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t *
     }
     for (int i = 0; i < kLanes; i++) CTX_CUDA(ctx, cudaStreamSynchronize(pl.lane[i].stream));
     if (result != LZ4B200_OK) return result;
-    CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_status, ctx->d_status.p, nb * 4, cudaMemcpyDeviceToHost, s0));
+    CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_status.p, ctx->d_status.p, nb * 4, cudaMemcpyDeviceToHost, s0));
     CTX_CUDA(ctx, cudaStreamSynchronize(s0));
-    memcpy(status, pl.h_status, nb * 4);
+    memcpy(status, pl.h_status.p, nb * 4);
     return LZ4B200_OK;
 }
 
@@ -1868,8 +1865,8 @@ static lz4b200_status decompress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t
     CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
     CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
     CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
-    CTX_CUDA(ctx, pinned_reserve(pl.h_seg, pl.h_seg_cap, (size_t)nb));
-    CTX_CUDA(ctx, pinned_reserve(pl.h_status, pl.h_status_cap, (size_t)nb * 2));
+    CTX_CUDA(ctx, pl.h_seg.reserve((size_t)nb));
+    CTX_CUDA(ctx, pl.h_status.reserve((size_t)nb * 2));
     cudaStream_t s0 = pl.lane[0].stream;
     CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_off.p, h_in_off.data(), nb * 8, cudaMemcpyHostToDevice, s0));
     CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_in_len.p, in_len, nb * 4, cudaMemcpyHostToDevice, s0));
@@ -1898,7 +1895,7 @@ static lz4b200_status decompress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t
                     ctx->d_out_cap.p + c.b0, ctx->d_out_len.p + c.b0, ctx->d_status.p + c.b0, ctx->d_expected.p + c.b0, n,
                     nullptr};
         if (dict_len) { a.dict = ctx->d_dict.p; a.dict_len = (uint32_t)dict_len; }
-        st = launch_decompress(ctx, a, ln.stream, pl.d_tickets + 8 * (ci % kLanes));
+        st = launch_decompress(ctx, a, ln.stream, pl.d_tickets.p + 8 * (ci % kLanes));
         if (st != LZ4B200_OK) return st;
         if (contiguous[ci]) {
             CTX_CUDA(ctx, cudaMemcpyAsync(out + c.a, ln.out.p, c.b - c.a, cudaMemcpyDeviceToHost, ln.stream));
@@ -1910,15 +1907,15 @@ static lz4b200_status decompress_batch_host_impl(lz4b200_ctx *ctx, const uint8_t
         }
     }
     for (int i = 0; i < kLanes; i++) CTX_CUDA(ctx, cudaStreamSynchronize(pl.lane[i].stream));
-    uint32_t *h_len = reinterpret_cast<uint32_t *>(pl.h_status + nb);
-    CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_status, ctx->d_status.p, nb * 4, cudaMemcpyDeviceToHost, s0));
+    uint32_t *h_len = reinterpret_cast<uint32_t *>(pl.h_status.p + nb);
+    CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_status.p, ctx->d_status.p, nb * 4, cudaMemcpyDeviceToHost, s0));
     CTX_CUDA(ctx, cudaMemcpyAsync(h_len, ctx->d_out_len.p, nb * 4, cudaMemcpyDeviceToHost, s0));
     if (err_expected)
-        CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_seg, ctx->d_expected.p, nb * 8, cudaMemcpyDeviceToHost, s0));
+        CTX_CUDA(ctx, cudaMemcpyAsync(pl.h_seg.p, ctx->d_expected.p, nb * 8, cudaMemcpyDeviceToHost, s0));
     CTX_CUDA(ctx, cudaStreamSynchronize(s0));
-    memcpy(status, pl.h_status, nb * 4);
+    memcpy(status, pl.h_status.p, nb * 4);
     memcpy(out_len, h_len, nb * 4);
-    if (err_expected) memcpy(err_expected, pl.h_seg, nb * 8);
+    if (err_expected) memcpy(err_expected, pl.h_seg.p, nb * 8);
     return LZ4B200_OK;
 }
 
@@ -2354,12 +2351,12 @@ lz4b200_status lz4b200_peer_alloc(lz4b200_ctx *ctx, size_t bytes, void **d_ptr, 
     if (!ctx || !d_ptr || !handle64 || !bytes) return LZ4B200_INVALID_ARGUMENT;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     DeviceGuard guard(ctx->device);
-    void *p = nullptr;
-    CTX_CUDA(ctx, cudaMalloc(&p, bytes));
+    DevBuf<uint8_t> buf;
+    CTX_CUDA(ctx, buf.resize(bytes));
     cudaIpcMemHandle_t h;
-    if (!ctx->check(cudaIpcGetMemHandle(&h, p), "cudaIpcGetMemHandle")) { cudaFree(p); return LZ4B200_CUDA_ERROR; }
+    if (!ctx->check(cudaIpcGetMemHandle(&h, buf.p), "cudaIpcGetMemHandle")) return LZ4B200_CUDA_ERROR;
     memcpy(handle64, &h, 64);
-    *d_ptr = p;
+    *d_ptr = std::exchange(buf.p, nullptr);
     return LZ4B200_OK;
 }
 
@@ -2623,7 +2620,7 @@ lz4b200_status decode_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *src
             // outputs
             BatchArgs l{src, ctx->d_in_off.p + nind, ctx->d_in_len.p + nind, nullptr, ctx->d_slots.p,
                         ctx->d_out_off.p + nind, ctx->d_out_cap.p + nind, ctx->d_out_len.p + nind,
-                        ctx->d_status.p + nind, ctx->d_expected.p + nind, nlnk, ctx->d_tickets};
+                        ctx->d_status.p + nind, ctx->d_expected.p + nind, nlnk, ctx->d_tickets.p};
             l.link_first = ctx->d_link_first.p + nind; l.stored_off = ctx->d_in_off.p + nind;
             l.stored_len = ctx->d_stored_len.p + nind; l.done = ctx->d_done.p + nind;
             lz4_decompress_blocks_linked<32><<<std::min<uint32_t>((nlnk + 3) / 4, (uint32_t)ctx->sm_count * 8), 128, 0, s>>>(l);
@@ -2977,9 +2974,9 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
 size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
 {
     if (!ctx) return 0;
-    size_t b = ctx->d_tickets ? 8 * sizeof(uint32_t) : 0;
+    size_t b = 0;
     auto add = [&b](const auto &buf) { b += buf.cap * sizeof(*buf.p); };
-    add(ctx->d_gtab16);
+    add(ctx->d_tickets); add(ctx->d_gtab16);
 #ifdef LZ4B200_AB_VARIANTS
     add(ctx->d_ttab16); add(ctx->d_gtag32);
 #endif
@@ -2991,9 +2988,9 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_bframe);
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
     add(ctx->d_gframe);
-    if (const Pipeline *p = static_cast<const Pipeline *>(ctx->pipe)) {
+    if (const Pipeline *p = ctx->pipe.get()) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
-        if (p->d_tickets) b += kMaxLanes * 8 * sizeof(uint32_t);
+        add(p->d_tickets);
     }
     return b;
 }
@@ -3144,7 +3141,7 @@ lz4b200_status lz4b200_frame_decoder_create(lz4b200_ctx *ctx, lz4b200_frame_deco
     dec->device = ctx->device;
     if (!ctx->check(dec->d_win.reserve(2 * kWindowBytes), "decoder window") ||
         !ctx->check(dec->d_content.reserve(1), "decoder content hash") || !ctx->check(dec->d_need.reserve(1), "decoder need")) {
-        lz4b200_frame_decoder_destroy(dec);
+        delete dec;
         return LZ4B200_CUDA_ERROR;
     }
     *out = dec;
@@ -3155,7 +3152,6 @@ void lz4b200_frame_decoder_destroy(lz4b200_frame_decoder *dec)
 {
     if (!dec) return;
     DeviceGuard guard(dec->device);
-    dec->d_win.release(); dec->d_content.release(); dec->d_need.release();
     delete dec;
 }
 
@@ -3182,8 +3178,7 @@ struct lz4b200_frame_encoder {
     int device = 0;
     lz4b200_frame_info info{};                // as created; the block size resolves into st
     fe::State st;
-    uint8_t *d_buf = nullptr;                 // the input buffer: st.group blocks of the open frame's block size
-    size_t buf_bytes = 0;
+    DevBuf<uint8_t> d_buf;                    // the input buffer: st.group blocks of the open frame's block size
     DevBuf<lz4b200_xxh32_state> d_content;    // the running content hash
     DevBuf<uint64_t> d_pos;                   // the call's output position, double-buffered: group g moves it from
                                               // d_pos[g % 2] to d_pos[(g + 1) % 2]
@@ -3203,7 +3198,7 @@ lz4b200_status lz4b200_frame_encoder_create(lz4b200_ctx *ctx, const lz4b200_fram
     enc->info = *info;
     enc->st.block_size_id = id;
     if (!ctx->check(enc->d_content.reserve(1), "encoder content hash") || !ctx->check(enc->d_pos.reserve(2), "encoder position")) {
-        lz4b200_frame_encoder_destroy(enc);
+        delete enc;
         return LZ4B200_CUDA_ERROR;
     }
     *out = enc;
@@ -3214,8 +3209,6 @@ void lz4b200_frame_encoder_destroy(lz4b200_frame_encoder *enc)
 {
     if (!enc) return;
     DeviceGuard guard(enc->device);
-    if (enc->d_buf) cudaFree(enc->d_buf);
-    enc->d_content.release(); enc->d_pos.release();
     delete enc;
 }
 
@@ -3243,13 +3236,8 @@ lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, c
     const fe::CallPlan p = fe::plan_call(enc->st, enc->info, ctx->frame_budget, n, op);
     const size_t bs = fe::block_bytes(p.block_size_id);
     const size_t want = p.group * bs;
-    if (p.header && want != enc->buf_bytes) {                // the buffer follows the block size and the budget
-        if (enc->d_buf) cudaFree(enc->d_buf);
-        enc->d_buf = nullptr;
-        enc->buf_bytes = 0;
-        CTX_CUDA(ctx, cudaMalloc(reinterpret_cast<void **>(&enc->d_buf), want));
-        enc->buf_bytes = want;
-    }
+    if (p.header && want != enc->d_buf.cap)                  // the buffer follows the block size and the budget
+        CTX_CUDA(ctx, enc->d_buf.resize(want));
 
     lz4b200_frame_info info = enc->info;
     info.block_size_id = p.block_size_id;
@@ -3265,16 +3253,16 @@ lz4b200_status lz4b200_frame_encoder_encode_device(lz4b200_frame_encoder *enc, c
     uint32_t g = 0;                                          // groups so far: the position is at pos[g % 2]
     for (const fe::Step &st : p.steps) {
         if (st.len)
-            CTX_CUDA(ctx, cudaMemcpyAsync(enc->d_buf + st.dst, d_in + st.src, st.len, cudaMemcpyDeviceToDevice, s));
+            CTX_CUDA(ctx, cudaMemcpyAsync(enc->d_buf.p + st.dst, d_in + st.src, st.len, cudaMemcpyDeviceToDevice, s));
         if (!st.group_len) continue;
         const fb::FramePlan plan = fe::group_plan(st, bs);
-        const lz4b200_status r = compress_frames(ctx, enc->d_buf, &plan, 1,
+        const lz4b200_status r = compress_frames(ctx, enc->d_buf.p, &plan, 1,
                                                  (uint32_t)std::min<uint64_t>(st.group_len, bs), info.block_checksums,
                                                  false, d_out, nullptr, pos + g % 2, pos + (g + 1) % 2, s);
         if (r != LZ4B200_OK) return r;
         g++;
         if (info.content_checksum) {                          // compress.rs:319-321, in stream order
-            content_hash_kernel<<<1, 256, 0, s>>>(enc->d_content.p, enc->d_buf, st.group_len);
+            content_hash_kernel<<<1, 256, 0, s>>>(enc->d_content.p, enc->d_buf.p, st.group_len);
             CTX_CUDA(ctx, cudaGetLastError());
         }
     }
