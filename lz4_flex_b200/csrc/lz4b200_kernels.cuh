@@ -21,10 +21,10 @@
 #define DEC_DEFER 1
 #endif
 #ifndef DEC_LIT_PRED
-#define DEC_LIT_PRED 0   // 1: fast-path literals as two predicated byte steps instead of a loop (A/B aid)
+#define DEC_LIT_PRED 1   // 1: fast-path literals as two predicated byte steps instead of a loop; 0: the loop (DESIGN.md §6)
 #endif
 #ifndef DEC_DEFER8
-#define DEC_DEFER8 0     // 1: deferred match stores cover 8 byte steps (64 bytes for G=8) instead of 4 (A/B aid)
+#define DEC_DEFER8 1     // 1: deferred match stores cover 8 byte steps (64 bytes for G=8); 0: 4 steps (DESIGN.md §6)
 #endif
 #ifndef DEC_PREFETCH
 #define DEC_PREFETCH 0   // > 0: K2 prefetches the compressed stream this many bytes ahead of the token cursor into L1 (build-time A/B)
@@ -386,7 +386,7 @@ __device__ __forceinline__ DecResult decode_block_simple(const uint8_t *__restri
     if (n == 0) { r.status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; return r; }   // decompress.rs:207-209
     const WordView view(src);
     uint32_t ip = 0, op = 0;
-    // deferral pays for 8-lane groups (4 byte-steps per match), not for wider ones
+    // deferral pays for 8-lane groups (8 byte-steps per match with DEC_DEFER8), not for wider ones
     constexpr bool kDefer = DEC_DEFER && G <= 8;
     uint8_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0;                // pending match bytes of this lane
 #if DEC_DEFER8
