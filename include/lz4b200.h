@@ -412,7 +412,13 @@ size_t lz4b200_frame_write_header(const lz4b200_frame_info *info, uint8_t *out, 
  * (decompress.rs:113-128), is a clean end: OK with *written == 0.
  *   - bytes decoded before a corrupt block / truncation are delivered (*written) together with the error;
  *   - *block_status receives the block decoder's code for FRAME_DECOMPRESSION_ERROR; *err_expected / *err_actual
- *     receive ContentLengthError{expected, actual} (frame/mod.rs) or the block's OutputTooSmall{expected, actual};
+ *     receive ContentLengthError{expected, actual} (frame/mod.rs) or the block's OutputTooSmall{expected, actual}.
+ *     OutputTooSmall is relative to the failing block on every frame path, linked frames included: expected = the
+ *     bytes the block had decoded + the literal run or match that did not fit, actual = the block size.  Two ways the
+ *     reference differs on linked frames, neither replicated: its decoder writes after the frame's earlier output in
+ *     one buffer, so its expected and actual also count that prefix (frame/decompress.rs:196-305); and once
+ *     that buffer has wrapped (an ext_dict window), a block decodes into the buffer's head and can pass the block
+ *     size without an error.  Here a block that decodes to more than the block size is always DEC_OUTPUT_TOO_SMALL;
  *   - frames with linked blocks (frame/decompress.rs:196-222, 277-305; what `lz4`, LZ4F and pyarrow write by
  *     default) are decoded too: their blocks form a dependency chain that the device resolves in stream order;
  *   - device memory is bounded: independent blocks are decoded in groups whose output slots
