@@ -478,6 +478,72 @@ lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx,
     uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
     lz4b200_frame_result *d_results, size_t nframes, void *stream);
 
+/* ---- random access into one frame in DEVICE memory (no lz4_flex counterpart) ------------------------------------------
+ * A frame records no decoded block sizes, so reading content bytes [a, b) of a frame means decoding it from its first
+ * block.  lz4b200_frame_index_device builds, on the GPU, the decoded offset and length of every block without decoding
+ * it; lz4b200_frame_decompress_ranges_device then decodes only the blocks that many byte ranges touch. */
+typedef struct lz4b200_frame_index_entry {
+    uint64_t payload_off;         /* the block's payload, from the frame's first byte */
+    uint64_t decoded_off;         /* the block's first content byte */
+    uint32_t word;                /* the BlockInfo word: payload length | 0x80000000 for a stored block */
+    uint32_t decoded_len;         /* the block's decoded bytes */
+} lz4b200_frame_index_entry;      /* 24 bytes */
+
+typedef struct lz4b200_frame_index_info {
+    uint64_t block_size;          /* the frame's maximum block size in bytes (8 MiB for legacy frames) */
+    uint64_t nblocks;             /* entries the index holds: the blocks before the first failing block */
+    uint64_t content_len;         /* their decoded total */
+    int32_t linked;               /* BlockMode::Linked */
+    int32_t pad;
+    lz4b200_frame_result result;  /* the frame's result, as lz4b200_frame_decompress_next_device returns it */
+} lz4b200_frame_index_info;       /* 72 bytes */
+
+/* Indexes the frame that starts at d_in[0] (the unit of lz4b200_frame_decompress_next_device).  The header and the
+ * BlockInfo chain are walked on the GPU, block checksums are verified there when the frame has them, and one GPU thread
+ * per block walks its token stream, reading only the compressed bytes: it makes every check the block decoder makes, in
+ * the same order, so a block it accepts decodes without error.  A device prefix sum then gives the decoded offsets.
+ *   - with d_index NULL the call only walks the chain and writes the blocks it records to *nblocks: a count to allocate
+ *     by.  Otherwise *nblocks receives the entries the call needs, the blocks before the first that fails its checksum;
+ *     with max_blocks below that the call returns INVALID_ARGUMENT having written only *nblocks.
+ *   - d_index[0, info->nblocks) receive the entries; entries past info->nblocks up to *nblocks may be written.
+ *   - info->result equals, field by field, what lz4b200_frame_decompress_next_device returns for the same bytes with a
+ *     sufficient cap, except that the content checksum is never verified (that needs every decoded byte): where that
+ *     call returns FRAME_CONTENT_CHECKSUM the index reports OK.  FRAME_CONTENT_LENGTH is reported.  info->content_len is
+ *     the device call's `written`: the decoded total of the indexed blocks.
+ *   - a linked frame's offsets that reach before a block are valid when they stay within the frame's earlier output;
+ *     the walk records how far each block reaches back and the check runs once the decoded offsets are known.
+ * The returned status is the call's own (INVALID_ARGUMENT, CUDA_ERROR) or OK; the frame's status is info->result.status.
+ * Work runs on `stream`, which the call synchronises; info and nblocks are host pointers, d_index device memory.
+ * The context's scratch holds a descriptor and the sizing results of every block while the call runs. */
+lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                          lz4b200_frame_index_entry *d_index, size_t max_blocks, size_t *nblocks,
+                                          lz4b200_frame_index_info *info, void *stream);
+
+/* Decodes content bytes [d_start[i], d_start[i] + d_len[i]) of the indexed frame at d_in[0, n) into
+ * d_out + d_out_off[i], for i < nranges, in one call.  Ranges are clipped to info->content_len like a Python slice, and
+ * d_written[i] receives the clipped length.  Nothing else of d_out is written; ranges may overlap each other in the
+ * frame, their outputs must not overlap (not checked).  Every array is in device memory; info is a host pointer.
+ *   - independent blocks: the blocks a range touches are found on the device by binary search over the decoded offsets.
+ *     A compressed block that lies wholly inside a range decodes straight into d_out; a range's partial first and last
+ *     blocks decode into context scratch and are copied out; stored blocks are copied.  Work goes in windows of blocks
+ *     whose scratch fits the frame budget (at least one block); ranges in chunks of 65 536.
+ *   - linked blocks: no random access.  Blocks [0, the last block any range touches] decode once, in stream order, in
+ *     groups that fit the frame budget, carrying the 64 KiB window from group to group as the streaming decoder does;
+ *     each range takes its slice as the decode passes it.  The cost is that of decoding the frame up to the furthest
+ *     range's end.
+ *   - the index is untrusted: its info and every entry are checked against n, the block size and each other before
+ *     anything is decoded (INVALID_ARGUMENT), and every decoded block must produce exactly its indexed length
+ *     (FRAME_DECOMPRESSION_ERROR; d_out's range regions then hold unspecified bytes).  Block checksums are not verified
+ *     again.
+ * INVALID_ARGUMENT before anything is enqueued: a null ctx or info, a null array with nranges > 0, a null d_in with
+ * n > 0, a null d_index with info->nblocks > 0.  Work runs on `stream`, which the call synchronises. */
+lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                                      const lz4b200_frame_index_info *info,
+                                                      const lz4b200_frame_index_entry *d_index,
+                                                      const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+                                                      const uint64_t *d_out_off, uint64_t *d_written, size_t nranges,
+                                                      void *stream);
+
 /* d_bound[f] = what lz4b200_frame_decoded_bound gives for region f when it holds one frame (the first frame's bound
  * when it holds several).  Enqueued on `stream`; the call returns without synchronising.  Argument errors as above. */
 lz4b200_status lz4b200_frame_decoded_bound_batch_device(lz4b200_ctx *ctx,

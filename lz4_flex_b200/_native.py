@@ -105,6 +105,11 @@ class FrameDecoderStepC(C.Structure):
                 ("pad", C.c_int32), ("result", FrameResultC)]
 
 
+class FrameIndexInfoC(C.Structure):
+    _fields_ = [("block_size", C.c_uint64), ("nblocks", C.c_uint64), ("content_len", C.c_uint64), ("linked", C.c_int32),
+                ("pad", C.c_int32), ("result", FrameResultC)]
+
+
 _lib = None
 
 _vp, _sz, _u32, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_int
@@ -166,6 +171,8 @@ SIGNATURES = {
     "lz4b200_frame_decoded_bound_device": (_i32, [_vp, _vp, _sz, _psz, _vp]),
     "lz4b200_frame_decompress_batch_device": (_i32, [_vp] * 8 + [_sz, _vp]),
     "lz4b200_frame_decoded_bound_batch_device": (_i32, [_vp] * 5 + [_sz, _vp]),
+    "lz4b200_frame_index_device": (_i32, [_vp, _vp, _sz, _vp, _sz, _psz, C.POINTER(FrameIndexInfoC), _vp]),
+    "lz4b200_frame_decompress_ranges_device": (_i32, [_vp, _vp, _sz, C.POINTER(FrameIndexInfoC)] + [_vp] * 6 + [_sz, _vp]),
     "lz4b200_ctx_set_frame_budget": (None, [_vp, _sz]),
     "lz4b200_ctx_device_bytes": (_sz, [_vp]),
     "lz4b200_frame_decoder_create": (_i32, [_vp, C.POINTER(_vp)]),

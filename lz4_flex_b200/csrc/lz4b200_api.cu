@@ -17,6 +17,7 @@
 
 #include "lz4b200_frame_batch.cuh"
 #include "lz4b200_frame_encoder.cuh"
+#include "lz4b200_frame_range.cuh"
 #include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
 #include "lz4b200_solo_kernel.cuh"
@@ -872,6 +873,11 @@ struct lz4b200_ctx {
     DevBuf<uint8_t> d_fhash;
     DevBuf<GroupFrame> d_gframe;              // the frames of a decode group
     DevBuf<fb::FramePlan> d_fplan;            // batch frame encoder: the host's plan, one entry per frame
+    // frame index and range decode: per block a linked block's reach; per range of a chunk its first block, block count
+    // and item offset; per item of a window the length its block must decode to; a linked frame's window and output
+    DevBuf<uint32_t> d_reach, d_rfirst, d_rcount, d_rwant;
+    DevBuf<uint64_t> d_ritem, d_rend;
+    DevBuf<uint8_t> d_rwin, d_rout;
 
     bool check(cudaError_t e, const char *what)
     {
@@ -2971,6 +2977,236 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
     return LZ4B200_OK;
 }
 
+// ---- frame index and range decode (no lz4_flex counterpart) ------------------------------------------------------------
+// The index: the one-frame device walk and block checksums, one sizing thread per block, then the frame decoders' own
+// result step (frame_resolve_kernel) over the sizes, so the index decides its result by the rules the decoders use.
+lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                          lz4b200_frame_index_entry *d_index, size_t max_blocks, size_t *nblocks,
+                                          lz4b200_frame_index_info *info, void *stream)
+{
+    if (!ctx || !nblocks || (!d_in && n) || (d_index && !info)) return LZ4B200_INVALID_ARGUMENT;
+    *nblocks = 0;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    fw::FrameWalk w;
+    std::vector<fw::FrameBlockDesc> blocks;
+    uint32_t bad = fw::kNoBlock;
+    lz4b200_status st = walk_frame_device(ctx, s, d_in, n, d_index != nullptr, w, blocks, &bad);
+    if (st != LZ4B200_OK) return st;
+    if (bad != fw::kNoBlock) {                               // the frame ends at the first block that fails its checksum
+        fw::frame_walk_fail_block(w, blocks[bad], bad);
+        blocks.resize(bad);
+    }
+    *nblocks = blocks.size();
+    if (!d_index) return LZ4B200_OK;
+    if (max_blocks < blocks.size() || blocks.size() >= 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    const uint32_t nb = (uint32_t)blocks.size(), grid = (nb + 127) / 128;
+    CTX_CUDA(ctx, ctx->d_walk.reserve(1)); CTX_CUDA(ctx, ctx->d_gframe.reserve(1)); CTX_CUDA(ctx, ctx->d_result.reserve(1));
+    CTX_CUDA(ctx, ctx->d_fhash.reserve(1)); CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_reach.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb + 1)); CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p, &w, sizeof w, cudaMemcpyHostToDevice, s));
+    if (nb) {
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_desc.p, blocks.data(), nb * sizeof(fw::FrameBlockDesc), cudaMemcpyHostToDevice, s));
+        fr::block_size_kernel<<<grid, 128, 0, s>>>(d_in, ctx->d_desc.p, nb, w.bs, w.linked != 0, ctx->d_out_len.p,
+                                                   ctx->d_status.p, ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_reach.p);
+        if (w.linked) {
+            scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_out_len.p, ctx->d_out_off.p, nb);
+            fr::block_reach_kernel<<<grid, 128, 0, s>>>(ctx->d_out_off.p, ctx->d_reach.p, nb, ctx->d_status.p,
+                                                        ctx->d_expected.p, ctx->d_out_len.p);
+        }
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    GroupFrame p{};
+    p.out_cap = ~0ull;                                        // a sufficient cap
+    p.walk = ctx->d_walk.p;
+    p.result = ctx->d_result.p;
+    p.nblocks = nb;
+    p.bad = fw::kNoBlock;
+    p.last = 1;
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_gframe.p, &p, sizeof p, cudaMemcpyHostToDevice, s));
+    frame_resolve_kernel<<<1, 128, 0, s>>>(ctx->d_gframe.p, 1, ctx->d_desc.p, ctx->d_out_len.p, ctx->d_status.p,
+                                           ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_gdst.p, ctx->d_glen.p, ctx->d_fhash.p);
+    if (nb) fr::index_entries_kernel<<<grid, 128, 0, s>>>(ctx->d_desc.p, ctx->d_gdst.p, ctx->d_glen.p, nb, d_index);
+    CTX_CUDA(ctx, cudaGetLastError());
+    lz4b200_frame_result r;
+    uint32_t failed = fw::kNoBlock;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&r, ctx->d_result.p, sizeof r, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(&failed, &ctx->d_gframe.p->bad, sizeof failed, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    *info = lz4b200_frame_index_info{};
+    info->block_size = w.bs;
+    info->nblocks = std::min(nb, failed);
+    info->content_len = r.written;
+    info->linked = w.linked;
+    info->result = r;
+    return LZ4B200_OK;
+}
+
+namespace {
+
+constexpr uint32_t kRangeChunk = 65536;                      // ranges planned per launch
+constexpr uint32_t kRangeItems = 65536;                      // (range, block) items per decode launch, at most
+
+// Independent blocks: per chunk of ranges, a plan (first block, block count, item offsets) and one readback of the item
+// count; then windows of items whose partial-block slots fit the frame budget, each decoded, checked and copied.
+lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in,
+                                         const lz4b200_frame_index_info &info, const lz4b200_frame_index_entry *d_index,
+                                         const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+                                         const uint64_t *d_out_off, uint64_t *d_written, uint32_t nr)
+{
+    const uint32_t nb = (uint32_t)info.nblocks;
+    const uint64_t slot = fw::slot_bytes(info.block_size);
+    const uint32_t K = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(kRangeItems, ctx->frame_budget / std::max<uint64_t>(slot, 1)));
+    CTX_CUDA(ctx, ctx->d_rfirst.reserve(kRangeChunk)); CTX_CUDA(ctx, ctx->d_rcount.reserve(kRangeChunk));
+    CTX_CUDA(ctx, ctx->d_ritem.reserve(kRangeChunk + 1));
+    CTX_CUDA(ctx, ctx->d_slots.reserve(K * slot + 16));
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(K)); CTX_CUDA(ctx, ctx->d_out_off.reserve(K)); CTX_CUDA(ctx, ctx->d_in_len.reserve(K));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(K)); CTX_CUDA(ctx, ctx->d_rwant.reserve(K)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(K));
+    CTX_CUDA(ctx, ctx->d_off_b.reserve(K)); CTX_CUDA(ctx, ctx->d_gdst.reserve(K)); CTX_CUDA(ctx, ctx->d_glen.reserve(K));
+    CTX_CUDA(ctx, ctx->d_pick.reserve(K)); CTX_CUDA(ctx, ctx->d_out_len.reserve(K)); CTX_CUDA(ctx, ctx->d_status.reserve(K));
+    fr::RangeItems a{d_index, info.content_len, d_start, d_len, d_out_off, 0, 0, ctx->d_rfirst.p, ctx->d_ritem.p,
+                     (uint64_t)(uintptr_t)ctx->d_slots.p - (uint64_t)(uintptr_t)d_out, slot,
+                     ctx->d_in_off.p, ctx->d_out_off.p, ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_rwant.p,
+                     ctx->d_seg_off.p, ctx->d_off_b.p, ctx->d_gdst.p, ctx->d_glen.p, ctx->d_pick.p};
+    for (uint32_t r0 = 0; r0 < nr; r0 += kRangeChunk) {
+        const uint32_t rc = std::min(kRangeChunk, nr - r0);
+        fr::range_plan_kernel<<<(rc + 127) / 128, 128, 0, s>>>(d_index, nb, info.content_len, d_start, d_len, d_written,
+                                                               r0, rc, ctx->d_rfirst.p, ctx->d_rcount.p);
+        scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_rcount.p, ctx->d_ritem.p, rc);
+        CTX_CUDA(ctx, cudaGetLastError());
+        uint64_t total = 0;
+        CTX_CUDA(ctx, cudaMemcpyAsync(&total, ctx->d_ritem.p + rc, sizeof total, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        a.r0 = r0;
+        a.rc = rc;
+        for (uint64_t j0 = 0; j0 < total; j0 += K) {
+            const uint32_t k = (uint32_t)std::min<uint64_t>(K, total - j0), grid = (k + 127) / 128;
+            fr::range_items_kernel<<<grid, 128, 0, s>>>(a, j0, k);
+            CTX_CUDA(ctx, cudaGetLastError());
+            BatchArgs b{d_in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, d_out, ctx->d_out_off.p, ctx->d_out_cap.p,
+                        ctx->d_out_len.p, ctx->d_status.p, nullptr, k, nullptr};
+            const lz4b200_status st = launch_decompress(ctx, b, s);
+            if (st != LZ4B200_OK) return st;
+            fr::range_check_kernel<<<grid, 128, 0, s>>>(ctx->d_rwant.p, ctx->d_out_len.p, ctx->d_status.p, k, ctx->d_bad.p);
+            GatherArgs g{ctx->d_slots.p, d_in, ctx->d_seg_off.p, ctx->d_off_b.p, ctx->d_glen.p, ctx->d_glen.p,
+                         ctx->d_pick.p, nullptr, d_out, ctx->d_gdst.p, k};
+            gather_segments_kernel<<<std::min<uint32_t>(k, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    return LZ4B200_OK;
+}
+
+// Linked blocks: blocks [0, the last one a range touches] in stream order, in groups that the group loop would not cut
+// (slots and input span within the frame budget), the 64 KiB window carried from group to group as the streaming
+// decoder carries it; after each group every range copies its part of the group's output.
+lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in,
+                                    const lz4b200_frame_index_info &info, const lz4b200_frame_index_entry *d_index,
+                                    const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+                                    const uint64_t *d_out_off, uint64_t *d_written, uint32_t nr)
+{
+    const uint32_t nb = (uint32_t)info.nblocks;
+    CTX_CUDA(ctx, ctx->d_rend.reserve(1));
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rend.p, 0, sizeof(uint64_t), s));
+    fr::range_end_kernel<<<(nr + 127) / 128, 128, 0, s>>>(d_start, d_len, info.content_len, d_written, nr,
+                                                          reinterpret_cast<unsigned long long *>(ctx->d_rend.p));
+    CTX_CUDA(ctx, cudaGetLastError());
+    uint64_t end = 0;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&end, ctx->d_rend.p, sizeof end, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    if (!end) return LZ4B200_OK;
+    std::vector<lz4b200_frame_index_entry> ent(nb);
+    CTX_CUDA(ctx, cudaMemcpyAsync(ent.data(), d_index, nb * sizeof(lz4b200_frame_index_entry), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    uint32_t last = 0;                                        // blocks [0, last) hold content [0, end)
+    while (last < nb && ent[last].decoded_off < end) last++;
+    CTX_CUDA(ctx, ctx->d_rwin.reserve(2 * kWindowBytes));
+    fw::FrameWalk w;                                          // what the group loop reads of the walk: a linked frame
+    w.bs = info.block_size;
+    w.linked = 1;
+    w.flg = 0;
+    w.stage = fw::kWalkDone;
+    uint32_t win = 0, win_len = 0;
+    uint64_t delivered = 0;
+    std::vector<fw::FrameBlockDesc> blocks;
+    for (uint32_t g0 = 0; g0 < last;) {
+        uint32_t g1 = g0;
+        uint64_t slots = 0, bytes = 0;
+        blocks.clear();
+        while (g1 < last) {
+            const fw::FrameBlockDesc d{ent[g1].payload_off, ent[g1].word, 0};
+            const uint64_t cap = fw::block_slot_cap(d, w.bs);
+            if (g1 > g0 && fw::group_cut(slots, cap, d.payload_off + fw::block_len(d) - blocks[0].payload_off, ctx->frame_budget))
+                break;
+            slots += fw::slot_bytes(cap);
+            bytes += ent[g1].decoded_len;
+            blocks.push_back(d);
+            g1++;
+        }
+        CTX_CUDA(ctx, ctx->d_rout.reserve(bytes + 16));
+        uint8_t *old = ctx->d_rwin.p + (size_t)win * kWindowBytes, *next = ctx->d_rwin.p + (size_t)(win ^ 1) * kWindowBytes;
+        lz4b200_frame_result r;
+        const lz4b200_status st = decode_frame_blocks(ctx, s, true, d_in, ctx->d_rout.p, bytes, w, blocks, false, delivered,
+                                                      nullptr, &r, nullptr, old, win_len);
+        if (st != LZ4B200_OK) return st;
+        if (r.status != LZ4B200_OK || r.written - delivered != bytes) return LZ4B200_FRAME_DECOMPRESSION_ERROR;
+        if (bytes) {
+            fr::range_slice_kernel<<<std::min<uint32_t>(nr, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(
+                ctx->d_rout.p, delivered, delivered + bytes, d_start, d_len, info.content_len, d_out, d_out_off, nr);
+            window_update_kernel<<<64, 256, 0, s>>>(old, win_len, ctx->d_rout.p, bytes, next);
+            CTX_CUDA(ctx, cudaGetLastError());
+            win ^= 1;
+            win_len = (uint32_t)std::min<uint64_t>(kWindowBytes, win_len + bytes);
+        }
+        delivered += bytes;
+        g0 = g1;
+    }
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
+                                                      const lz4b200_frame_index_info *info,
+                                                      const lz4b200_frame_index_entry *d_index,
+                                                      const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+                                                      const uint64_t *d_out_off, uint64_t *d_written, size_t nranges,
+                                                      void *stream)
+{
+    if (!ctx || !info || (!d_in && n) || nranges > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (nranges && (!d_start || !d_len || !d_out || !d_out_off || !d_written)) return LZ4B200_INVALID_ARGUMENT;
+    // the info is checked before anything of the index is read: a block size the format allows, a block count the
+    // planner can index, a content length the blocks can hold
+    const uint64_t bs = info->block_size, nbx = info->nblocks;
+    const bool bs_ok = bs == (64u << 10) || bs == (256u << 10) || bs == (1u << 20) || bs == (4u << 20) || bs == (8u << 20);
+    if (nbx >= 0xffffffffull || (nbx && (!d_index || !bs_ok)) || info->content_len > nbx * bs)
+        return LZ4B200_INVALID_ARGUMENT;
+    if (!nranges) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t nb = (uint32_t)nbx, nr = (uint32_t)nranges;
+    CTX_CUDA(ctx, ctx->d_bad.reserve(1));
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bad.p, 0, 4, s));
+    uint32_t bad = 0;
+    if (nb) {
+        fr::index_check_kernel<<<(nb + 255) / 256, 256, 0, s>>>(d_index, nb, n, bs, info->content_len, ctx->d_bad.p);
+        CTX_CUDA(ctx, cudaGetLastError());
+        CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        if (bad) return LZ4B200_INVALID_ARGUMENT;
+    }
+    const lz4b200_status st = info->linked
+        ? decode_ranges_linked(ctx, s, d_in, *info, d_index, d_start, d_len, d_out, d_out_off, d_written, nr)
+        : decode_ranges_independent(ctx, s, d_in, *info, d_index, d_start, d_len, d_out, d_out_off, d_written, nr);
+    if (st == LZ4B200_CUDA_ERROR) return st;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    if (st != LZ4B200_OK) return st;
+    return bad ? LZ4B200_FRAME_DECOMPRESSION_ERROR : LZ4B200_OK;
+}
+
 size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
 {
     if (!ctx) return 0;
@@ -2987,7 +3223,8 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_status); add(ctx->d_walk); add(ctx->d_desc); add(ctx->d_bad); add(ctx->d_content); add(ctx->d_result);
     add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_bframe);
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
-    add(ctx->d_gframe);
+    add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
+    add(ctx->d_rend); add(ctx->d_rwin); add(ctx->d_rout);
     if (const Pipeline *p = ctx->pipe.get()) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
         add(p->d_tickets);

@@ -25,7 +25,8 @@ from typing import Optional
 import numpy as np
 
 from . import _native, block as _block
-from .errors import (ContentChecksumError, ContentLengthError, IoError, LinkedBlocksUnsupported, error_from_status)
+from .errors import (ContentChecksumError, ContentLengthError, DecompressionError, IoError, LinkedBlocksUnsupported,
+                     error_from_status)
 
 WINDOW_SIZE = 64 * 1024
 _REPOSITION_LIMIT = 0xFFFFFFFF // 2          # u32::MAX as usize / 2  (frame/compress.rs:266)
@@ -399,6 +400,101 @@ def decompress_frames_device(d_in, offsets, lengths, out=None, out_offsets=None,
     if st != 0:
         raise error_from_status(st, detail=ctx.last_cuda_error())
     return DecodedFrames(out, oo, results)
+
+
+_CONTENT_CHECKSUM = 108
+
+
+@dataclass
+class FrameIndex:
+    """What index_frame_device() returns for one frame: its result, and one row per block it covers as an int64 CUDA
+    tensor of shape (nblocks, 3) holding lz4b200_frame_index_entry: payload offset, decoded offset, and the BlockInfo
+    word | decoded length << 32.  Blocks are those before the first failing block; `error` is the exception
+    decompress_next_frame_device() would raise for the frame, except that the content checksum is not verified."""
+    consumed: int
+    content_len: int
+    nblocks: int
+    block_size: int
+    linked: bool
+    error: Optional[Exception]
+    entries: "object"
+    _info: "object" = None
+
+    def decoded_lengths(self):
+        return self.entries[:, 2] >> 32 if self.nblocks else self.entries[:, 2]
+
+
+def index_frame_device(d_in, ctx: _block.Context | None = None, stream: int | None = None) -> FrameIndex:
+    """Indexes the frame that starts at the device tensor d_in[0] (lz4b200_frame_index_device): the decoded offset and
+    length of every block, found on the GPU without decoding, for decompress_ranges_device()."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
+    L = _native.lib()
+    n = d_in.numel()
+    ptr = d_in.data_ptr() if n else None
+    count, info = C.c_size_t(0), _native.FrameIndexInfoC()
+    st = L.lz4b200_frame_index_device(ctx.handle, ptr, n, None, 0, C.byref(count), None, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    entries = torch.empty((max(count.value, 1), 3), dtype=torch.int64, device=d_in.device)
+    st = L.lz4b200_frame_index_device(ctx.handle, ptr, n, entries.data_ptr(), count.value, C.byref(count),
+                                      C.byref(info), s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    r = info.result
+    err = None if r.status in (0, _CONTENT_CHECKSUM) else error_from_status(r.status, r.block_status, "", r.err_expected,
+                                                                            r.err_actual)
+    return FrameIndex(r.consumed, info.content_len, info.nblocks, info.block_size, bool(info.linked), err,
+                      entries[:info.nblocks], info)
+
+
+def decompress_ranges_device(d_in, index: FrameIndex, starts, lengths, out=None, out_offsets=None,
+                             ctx: _block.Context | None = None, stream: int | None = None):
+    """Content bytes [starts[i], starts[i] + lengths[i]) of the frame `index` describes, for every i, decoded from the
+    device tensor d_in in one call (lz4b200_frame_decompress_ranges_device).  Ranges are clipped to index.content_len
+    like Python slices.  Range i goes to out[out_offsets[i]:]; with out=None the ranges are laid back to back (lengths
+    are read on the host to size `out`).  Only the blocks a range touches are decoded (a linked frame decodes from its
+    first block).  Returns (out, out_offsets, written): CUDA int64 tensors, written[i] the clipped length of range i.
+    Raises InvalidArgument for an index that does not fit the bytes, and DecompressionError when a block does not decode
+    to its indexed length."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    st_t, ln_t = _device_i64(starts, dev, "starts"), _device_i64(lengths, dev, "lengths")
+    nr = st_t.numel()
+    if ln_t.numel() != nr:
+        raise ValueError("starts and lengths differ in length")
+    if (out is None) != (out_offsets is None):
+        raise ValueError("out and out_offsets go together")
+    if out is None:
+        a, b = _host_i64(starts, "starts"), _host_i64(lengths, "lengths")
+        c = index.content_len
+        s0 = np.minimum(a, c)
+        clipped = np.minimum(b, c - s0)
+        ends = np.cumsum(clipped)
+        oo = torch.as_tensor(ends - clipped, dtype=torch.int64).to(dev)
+        out = torch.empty(max(int(ends[-1]) if nr else 0, 1), dtype=torch.uint8, device=dev)
+    else:
+        _device_u8(out, "out")
+        oo = _device_i64(out_offsets, dev, "out_offsets")
+        if oo.numel() != nr:
+            raise ValueError("out_offsets needs one entry per range")
+    written = torch.zeros(nr, dtype=torch.int64, device=dev)
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    st = _native.lib().lz4b200_frame_decompress_ranges_device(
+        ctx.handle, d_in.data_ptr() if d_in.numel() else None, d_in.numel(), C.byref(index._info),
+        index.entries.data_ptr() if index.nblocks else None, st_t.data_ptr(), ln_t.data_ptr(), out.data_ptr(),
+        oo.data_ptr(), written.data_ptr(), nr, s)
+    if st == 101:
+        raise DecompressionError(ValueError("a block does not decode to its indexed length"))
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return out, oo, written
 
 
 class DeviceFrameDecoder:
