@@ -527,10 +527,14 @@ lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in,
  *     A compressed block that lies wholly inside a range decodes straight into d_out; a range's partial first and last
  *     blocks decode into context scratch and are copied out; stored blocks are copied.  Work goes in windows of blocks
  *     whose scratch fits the frame budget (at least one block); ranges in chunks of 65 536.
- *   - linked blocks: no random access.  Blocks [0, the last block any range touches] decode once, in stream order, in
- *     groups that fit the frame budget, carrying the 64 KiB window from group to group as the streaming decoder does;
- *     each range takes its slice as the decode passes it.  The cost is that of decoding the frame up to the furthest
- *     range's end.
+ *   - linked blocks: the touched blocks form segments of consecutive blocks, each with a look-back of the blocks that
+ *     hold the 64 KiB of content before it.  A segment's blocks decode in parallel without their window: each output
+ *     byte is its value or a marker naming the earlier byte it copies.  Markers then resolve in block order.  A segment
+ *     with a requested byte that copies content before its look-back decodes again with the look-back doubled (in
+ *     blocks), up to block 0; segments whose look-backs meet merge.  On English text (dickens, 64 KiB blocks) the
+ *     look-back stays 2-4 blocks; on data that copies itself from block to block (a file tiled over and over, such as
+ *     repeated JSON or logs) it reaches block 0.  Entries take four bytes per content byte, in windows that fit the
+ *     frame budget (at least one block and 64 KiB of carry).
  *   - the index is untrusted: its info and every entry are checked against n, the block size and each other before
  *     anything is decoded (INVALID_ARGUMENT), and every decoded block must produce exactly its indexed length
  *     (FRAME_DECOMPRESSION_ERROR; d_out's range regions then hold unspecified bytes).  Block checksums are not verified
@@ -543,6 +547,11 @@ lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const ui
                                                       const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
                                                       const uint64_t *d_out_off, uint64_t *d_written, size_t nranges,
                                                       void *stream);
+
+/* Block decodes the context's last lz4b200_frame_decompress_ranges_device call ran: for a linked frame every block of
+ * every round, look-back included; for independent blocks the (range, block) items.  0 after a call that decoded
+ * nothing.  A diagnostic: it shows how far random access into a frame reached back. */
+uint64_t lz4b200_ctx_last_range_blocks(const lz4b200_ctx *ctx);
 
 /* d_bound[f] = what lz4b200_frame_decoded_bound gives for region f when it holds one frame (the first frame's bound
  * when it holds several).  Enqueued on `stream`; the call returns without synchronising.  Argument errors as above. */

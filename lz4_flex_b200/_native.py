@@ -173,6 +173,7 @@ SIGNATURES = {
     "lz4b200_frame_decoded_bound_batch_device": (_i32, [_vp] * 5 + [_sz, _vp]),
     "lz4b200_frame_index_device": (_i32, [_vp, _vp, _sz, _vp, _sz, _psz, C.POINTER(FrameIndexInfoC), _vp]),
     "lz4b200_frame_decompress_ranges_device": (_i32, [_vp, _vp, _sz, C.POINTER(FrameIndexInfoC)] + [_vp] * 6 + [_sz, _vp]),
+    "lz4b200_ctx_last_range_blocks": (C.c_uint64, [_vp]),
     "lz4b200_ctx_set_frame_budget": (None, [_vp, _sz]),
     "lz4b200_ctx_device_bytes": (_sz, [_vp]),
     "lz4b200_frame_decoder_create": (_i32, [_vp, C.POINTER(_vp)]),

@@ -874,10 +874,16 @@ struct lz4b200_ctx {
     DevBuf<GroupFrame> d_gframe;              // the frames of a decode group
     DevBuf<fb::FramePlan> d_fplan;            // batch frame encoder: the host's plan, one entry per frame
     // frame index and range decode: per block a linked block's reach; per range of a chunk its first block, block count
-    // and item offset; per item of a window the length its block must decode to; a linked frame's window and output
+    // and item offset; per item of a window the length its block must decode to.  Linked frames: the touched blocks'
+    // difference array, a window's marker entries, blocks and pieces, the carry from window to window, and per segment
+    // of a round whether a requested byte stayed unresolved
     DevBuf<uint32_t> d_reach, d_rfirst, d_rcount, d_rwant;
-    DevBuf<uint64_t> d_ritem, d_rend;
-    DevBuf<uint8_t> d_rwin, d_rout;
+    DevBuf<uint64_t> d_ritem;
+    DevBuf<int32_t> d_rtouch;
+    DevBuf<uint32_t> d_rent, d_rcarry, d_rflag;
+    DevBuf<fr::MarkBlock> d_rblk;
+    DevBuf<fr::MarkPiece> d_rpiece;
+    uint64_t last_range_blocks = 0;           // block decodes of the last ranges call (lz4b200_ctx_last_range_blocks)
 
     bool check(cudaError_t e, const char *what)
     {
@@ -3079,6 +3085,7 @@ lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const
         uint64_t total = 0;
         CTX_CUDA(ctx, cudaMemcpyAsync(&total, ctx->d_ritem.p + rc, sizeof total, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        ctx->last_range_blocks += total;
         a.r0 = r0;
         a.rc = rc;
         for (uint64_t j0 = 0; j0 < total; j0 += K) {
@@ -3099,69 +3106,134 @@ lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const
     return LZ4B200_OK;
 }
 
-// Linked blocks: blocks [0, the last one a range touches] in stream order, in groups that the group loop would not cut
-// (slots and input span within the frame budget), the 64 KiB window carried from group to group as the streaming
-// decoder carries it; after each group every range copies its part of the group's output.
+// Linked blocks: segments of consecutive touched blocks, each with a look-back of the blocks that hold the 64 KiB of
+// content before it.  A round marker-decodes every active segment's blocks (look-back included) in windows of entries
+// that fit the frame budget, resolves them and copies the ranges out; a segment with a requested byte still unresolved
+// doubles its look-back (in blocks) for the next round, and segments whose look-backs meet merge.  A segment that starts
+// at block 0 always resolves: a byte that copies content before byte 0 fails its block.
+struct LinkedSeg {
+    uint32_t j, a, b;                         // decoded blocks [j, b]; the ranges touch blocks [a, b]
+};
+
 lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in,
                                     const lz4b200_frame_index_info &info, const lz4b200_frame_index_entry *d_index,
                                     const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
                                     const uint64_t *d_out_off, uint64_t *d_written, uint32_t nr)
 {
     const uint32_t nb = (uint32_t)info.nblocks;
-    CTX_CUDA(ctx, ctx->d_rend.reserve(1));
-    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rend.p, 0, sizeof(uint64_t), s));
-    fr::range_end_kernel<<<(nr + 127) / 128, 128, 0, s>>>(d_start, d_len, info.content_len, d_written, nr,
-                                                          reinterpret_cast<unsigned long long *>(ctx->d_rend.p));
+    CTX_CUDA(ctx, ctx->d_rtouch.reserve(nb + 1));
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rtouch.p, 0, (nb + 1) * sizeof(int32_t), s));
+    fr::range_touch_kernel<<<(nr + 127) / 128, 128, 0, s>>>(d_index, nb, info.content_len, d_start, d_len, d_written, nr,
+                                                            ctx->d_rtouch.p);
     CTX_CUDA(ctx, cudaGetLastError());
-    uint64_t end = 0;
-    CTX_CUDA(ctx, cudaMemcpyAsync(&end, ctx->d_rend.p, sizeof end, cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaStreamSynchronize(s));
-    if (!end) return LZ4B200_OK;
+    std::vector<int32_t> touch(nb + 1);
     std::vector<lz4b200_frame_index_entry> ent(nb);
+    CTX_CUDA(ctx, cudaMemcpyAsync(touch.data(), ctx->d_rtouch.p, (nb + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     CTX_CUDA(ctx, cudaMemcpyAsync(ent.data(), d_index, nb * sizeof(lz4b200_frame_index_entry), cudaMemcpyDeviceToHost, s));
     CTX_CUDA(ctx, cudaStreamSynchronize(s));
-    uint32_t last = 0;                                        // blocks [0, last) hold content [0, end)
-    while (last < nb && ent[last].decoded_off < end) last++;
-    CTX_CUDA(ctx, ctx->d_rwin.reserve(2 * kWindowBytes));
-    fw::FrameWalk w;                                          // what the group loop reads of the walk: a linked frame
-    w.bs = info.block_size;
-    w.linked = 1;
-    w.flg = 0;
-    w.stage = fw::kWalkDone;
-    uint32_t win = 0, win_len = 0;
-    uint64_t delivered = 0;
-    std::vector<fw::FrameBlockDesc> blocks;
-    for (uint32_t g0 = 0; g0 < last;) {
-        uint32_t g1 = g0;
-        uint64_t slots = 0, bytes = 0;
-        blocks.clear();
-        while (g1 < last) {
-            const fw::FrameBlockDesc d{ent[g1].payload_off, ent[g1].word, 0};
-            const uint64_t cap = fw::block_slot_cap(d, w.bs);
-            if (g1 > g0 && fw::group_cut(slots, cap, d.payload_off + fw::block_len(d) - blocks[0].payload_off, ctx->frame_budget))
-                break;
-            slots += fw::slot_bytes(cap);
-            bytes += ent[g1].decoded_len;
-            blocks.push_back(d);
-            g1++;
+    // the last block whose decoded offset is at most x, as fr::block_at finds it
+    auto block_at = [&](uint64_t x) {
+        uint32_t lo = 0, hi = nb;
+        while (hi - lo > 1) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            if (ent[mid].decoded_off <= x) lo = mid; else hi = mid;
         }
-        CTX_CUDA(ctx, ctx->d_rout.reserve(bytes + 16));
-        uint8_t *old = ctx->d_rwin.p + (size_t)win * kWindowBytes, *next = ctx->d_rwin.p + (size_t)(win ^ 1) * kWindowBytes;
-        lz4b200_frame_result r;
-        const lz4b200_status st = decode_frame_blocks(ctx, s, true, d_in, ctx->d_rout.p, bytes, w, blocks, false, delivered,
-                                                      nullptr, &r, nullptr, old, win_len);
-        if (st != LZ4B200_OK) return st;
-        if (r.status != LZ4B200_OK || r.written - delivered != bytes) return LZ4B200_FRAME_DECOMPRESSION_ERROR;
-        if (bytes) {
-            fr::range_slice_kernel<<<std::min<uint32_t>(nr, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(
-                ctx->d_rout.p, delivered, delivered + bytes, d_start, d_len, info.content_len, d_out, d_out_off, nr);
-            window_update_kernel<<<64, 256, 0, s>>>(old, win_len, ctx->d_rout.p, bytes, next);
+        return lo;
+    };
+    std::vector<LinkedSeg> act;
+    int32_t run = 0;
+    for (uint32_t b = 0; b < nb; b++) {
+        run += touch[b];
+        if (run <= 0) continue;
+        if (!act.empty() && act.back().b + 1 == b) { act.back().b = b; continue; }
+        const uint64_t d = ent[b].decoded_off;
+        act.push_back({d > fr::kCarry ? block_at(d - fr::kCarry) : 0u, b, b});
+    }
+    const uint64_t window = std::min<uint64_t>(std::max<uint64_t>(ctx->frame_budget / 4, fr::kCarry + info.block_size),
+                                               1u << 30);
+    const uint32_t sms = (uint32_t)ctx->sm_count;
+    CTX_CUDA(ctx, ctx->d_rcarry.reserve(fr::kCarry));
+    uint64_t decodes = 0;
+    ctx->last_range_blocks = 0;
+    std::vector<fr::MarkBlock> blk;
+    std::vector<fr::MarkPiece> piece;
+    struct Win { uint32_t blk0, blk1, p0, p1; uint64_t entries; };
+    std::vector<Win> wins;
+    while (!act.empty()) {
+        std::vector<LinkedSeg> m;                                  // merge segments whose look-backs meet
+        for (const LinkedSeg &g : act) {
+            if (!m.empty() && g.j <= m.back().b + 1) { m.back().j = std::min(m.back().j, g.j); m.back().b = g.b; }
+            else m.push_back(g);
+        }
+        act.swap(m);
+        // the round's windows: each segment's blocks in order, a piece per segment and window
+        blk.clear(); piece.clear(); wins.clear();
+        uint64_t used = 0;
+        wins.push_back({0, 0, 0, 0, 0});
+        for (uint32_t g = 0; g < act.size(); g++) {
+            bool carried = false;
+            for (uint32_t k = act[g].j; k <= act[g].b;) {
+                if (used && used + fr::kCarry + ent[k].decoded_len > window) {   // a new window
+                    wins.back().blk1 = (uint32_t)blk.size(); wins.back().p1 = (uint32_t)piece.size();
+                    wins.back().entries = used;
+                    wins.push_back({(uint32_t)blk.size(), 0, (uint32_t)piece.size(), 0, 0});
+                    used = 0;
+                }
+                fr::MarkPiece p{ent[k].decoded_off, ent[k].decoded_off, ent[act[g].a].decoded_off, (uint32_t)blk.size(),
+                                0, (uint32_t)used, g, carried ? 1u : 0u, 0};
+                used += fr::kCarry;
+                do {
+                    blk.push_back({ent[k].payload_off, ent[k].decoded_off, ent[k].word, ent[k].decoded_len, (uint32_t)used});
+                    used += ent[k].decoded_len;
+                    p.c1 += ent[k].decoded_len;
+                    k++;
+                } while (k <= act[g].b && used + ent[k].decoded_len <= window);
+                p.blk1 = (uint32_t)blk.size();
+                piece.push_back(p);
+                carried = true;
+            }
+        }
+        wins.back().blk1 = (uint32_t)blk.size(); wins.back().p1 = (uint32_t)piece.size(); wins.back().entries = used;
+        uint64_t most = 0;
+        for (const Win &w : wins) most = std::max(most, w.entries);
+        CTX_CUDA(ctx, ctx->d_rent.reserve(most));
+        CTX_CUDA(ctx, ctx->d_rblk.reserve(blk.size())); CTX_CUDA(ctx, ctx->d_rpiece.reserve(piece.size()));
+        CTX_CUDA(ctx, ctx->d_rflag.reserve(act.size()));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_rblk.p, blk.data(), blk.size() * sizeof(fr::MarkBlock), cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_rpiece.p, piece.data(), piece.size() * sizeof(fr::MarkPiece), cudaMemcpyHostToDevice, s));
+        CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rflag.p, 0, act.size() * sizeof(uint32_t), s));
+        for (const Win &w : wins) {
+            const uint32_t k = w.blk1 - w.blk0, np = w.p1 - w.p0;
+            fr::marker_decode_kernel<32><<<(k + 3) / 4, 128, 0, s>>>(d_in, ctx->d_rblk.p + w.blk0, k, ctx->d_rent.p,
+                                                                    ctx->d_bad.p);
+            fr::resolve_tails_kernel<<<np, 1024, 0, s>>>(ctx->d_rblk.p, ctx->d_rpiece.p + w.p0, ctx->d_rcarry.p,
+                                                         ctx->d_rent.p);
+            fr::entries_out_kernel<<<std::min<uint32_t>(nr, sms * 8), 256, 0, s>>>(
+                ctx->d_rent.p, ctx->d_rpiece.p + w.p0, np, d_start, d_len, info.content_len, d_out, d_out_off, nr,
+                ctx->d_rflag.p);
             CTX_CUDA(ctx, cudaGetLastError());
-            win ^= 1;
-            win_len = (uint32_t)std::min<uint64_t>(kWindowBytes, win_len + bytes);
+            const fr::MarkPiece &last = piece[w.p1 - 1];           // a segment cut here carries its last 64 KiB on
+            if (w.p1 < piece.size() && piece[w.p1].carried)
+                CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_rcarry.p, ctx->d_rent.p + last.base + (last.c1 - last.c0),
+                                              fr::kCarry * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+            decodes += k;
         }
-        delivered += bytes;
-        g0 = g1;
+        std::vector<uint32_t> flag(act.size());
+        uint32_t bad = 0;
+        CTX_CUDA(ctx, cudaMemcpyAsync(flag.data(), ctx->d_rflag.p, act.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        ctx->last_range_blocks = decodes;
+        if (bad) return LZ4B200_FRAME_DECOMPRESSION_ERROR;
+        m.clear();
+        for (uint32_t g = 0; g < act.size(); g++) {
+            if (!flag[g]) continue;
+            const LinkedSeg &x = act[g];
+            if (x.j == 0) return LZ4B200_FRAME_DECOMPRESSION_ERROR;   // cannot happen: such bytes fail their block
+            const uint32_t back = 2 * (x.a - x.j);
+            m.push_back({back >= x.a ? 0u : x.a - back, x.a, x.b});
+        }
+        act.swap(m);
     }
     return LZ4B200_OK;
 }
@@ -3177,6 +3249,7 @@ lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const ui
 {
     if (!ctx || !info || (!d_in && n) || nranges > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
     if (nranges && (!d_start || !d_len || !d_out || !d_out_off || !d_written)) return LZ4B200_INVALID_ARGUMENT;
+    ctx->last_range_blocks = 0;
     // the info is checked before anything of the index is read: a block size the format allows, a block count the
     // planner can index, a content length the blocks can hold
     const uint64_t bs = info->block_size, nbx = info->nblocks;
@@ -3207,6 +3280,11 @@ lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const ui
     return bad ? LZ4B200_FRAME_DECOMPRESSION_ERROR : LZ4B200_OK;
 }
 
+uint64_t lz4b200_ctx_last_range_blocks(const lz4b200_ctx *ctx)
+{
+    return ctx ? ctx->last_range_blocks : 0;
+}
+
 size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
 {
     if (!ctx) return 0;
@@ -3224,7 +3302,7 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_bframe);
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
     add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
-    add(ctx->d_rend); add(ctx->d_rwin); add(ctx->d_rout);
+    add(ctx->d_rtouch); add(ctx->d_rent); add(ctx->d_rcarry); add(ctx->d_rflag); add(ctx->d_rblk); add(ctx->d_rpiece);
     if (const Pipeline *p = ctx->pipe.get()) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
         add(p->d_tickets);

@@ -11,6 +11,7 @@
 
 #include "../../include/lz4b200.h"
 #include "lz4b200_frame_walk.cuh"
+#include "lz4b200_kernels.cuh"
 
 namespace lz4b200 {
 namespace fr {
@@ -231,32 +232,191 @@ __global__ void __launch_bounds__(128) range_check_kernel(const uint32_t *want, 
     if (status[t] != LZ4B200_OK || out_len[t] != want[t]) atomicOr(bad, 1u);
 }
 
-// Linked frames: the clipped end of the furthest range, into *end (atomicMax).
-__global__ void __launch_bounds__(128) range_end_kernel(const uint64_t *start, const uint64_t *len, uint64_t content_len,
-                                                        uint64_t *written, uint32_t nr, unsigned long long *end)
+// ---- linked frames: marker decode ------------------------------------------------------------------------------------
+// A block of a linked frame decodes without the 64 KiB of content before it when every output byte is an entry: the
+// byte's value, or a marker naming the earlier entry it copies because its match reaches before the block.  A value
+// depends only on compressed bytes, so it is the byte the whole-frame decode gives.  The blocks of a segment (consecutive
+// blocks, from a look-back before the blocks the ranges touch) decode in parallel into a window of entries, then markers
+// resolve in block order: every marker of a block names one of the 65 535 entries before the block's first, which lie in
+// the last 64 KiB of the blocks before it.  Each segment's piece of a window starts with 64 KiB of carry entries: the end
+// of the segment's previous piece, or poison for its first.  A byte still poison after resolving copies content before
+// the segment, and the segment's look-back is too short.
+constexpr uint32_t kMark = 0x80000000u;      // | the window index of the entry a byte copies
+constexpr uint32_t kPoison = 0xffffffffu;    // a byte that copies content before its segment
+constexpr uint32_t kCarry = 65536;           // carry entries in front of each piece
+
+struct MarkBlock {
+    uint64_t payload_off, decoded_off;       // from the index
+    uint32_t word, len;                      // BlockInfo word, indexed decoded length
+    uint32_t at;                             // its first entry in the window
+};
+
+struct MarkPiece {                           // one segment's blocks in one window
+    uint64_t c0, c1;                         // content [c0, c1)
+    uint64_t t0;                             // the segment's first touched byte: its ranges start here or later
+    uint32_t blk0, blk1;                     // its blocks in the window's MarkBlock list
+    uint32_t base;                           // its carry entries: [base, base + kCarry); its blocks follow
+    uint32_t seg;                            // the segment, for the unresolved flag
+    uint32_t carried;                        // 1: the carry is the previous window's last piece's end (in carry[])
+    uint32_t pad;
+};
+
+// One G-lane group per block: the checks of decode_block_linked in the same order, on entries.  Stored blocks are
+// values.  A match that reaches before the block's first byte writes markers for that part (its reach before content
+// byte 0 is OffsetOutOfBounds, as in the decoder); the rest copies entries with the byte-serial semantics of copy_match,
+// so a marker copied inside the block still names an entry before the block.  A block that fails or does not produce
+// exactly its indexed length sets *bad.
+template <int G>
+__global__ void __launch_bounds__(128) marker_decode_kernel(const uint8_t *in, const MarkBlock *blocks, uint32_t nb,
+                                                            uint32_t *ent, uint32_t *bad)
+{
+    const uint32_t lane = threadIdx.x & 31u, sub = lane & (G - 1), leader = lane & ~uint32_t(G - 1);
+    const uint32_t gmask = G == 32 ? kFull : (((1u << (G & 31)) - 1u) << leader);
+    const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) / G;
+    if (b >= nb) return;
+    const MarkBlock bk = blocks[b];
+    const uint8_t *__restrict__ src = in + bk.payload_off;
+    uint32_t *dst = ent + bk.at;
+    const uint32_t n = bk.word & 0x7fffffffu, cap = bk.len;
+    if (bk.word & 0x80000000u) {                                   // stored: len == n (checked with the index)
+        for (uint32_t i = sub; i < cap; i += G) dst[i] = __ldg(src + i);
+        return;
+    }
+    int32_t status = LZ4B200_OK;
+    uint32_t ip = 0, op = 0;
+    if (n == 0) status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE;
+    while (status == LZ4B200_OK) {
+        const uint32_t tok = __ldg(src + ip++);
+        uint64_t lit = tok >> 4;
+        if (lit == 15) {
+            for (;;) {
+                if (ip >= n) { status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; break; }
+                const uint32_t v = __ldg(src + ip++);
+                lit += v;
+                if (v != 255) break;
+            }
+            if (status != LZ4B200_OK) break;
+        }
+        if (lit) {
+            if (lit > (uint64_t)(n - ip)) { status = LZ4B200_DEC_LITERAL_OUT_OF_BOUNDS; break; }
+            if (lit > (uint64_t)(cap - op)) { status = LZ4B200_DEC_OUTPUT_TOO_SMALL; break; }
+            for (uint32_t i = sub; i < (uint32_t)lit; i += G) dst[op + i] = __ldg(src + ip + i);
+            ip += (uint32_t)lit; op += (uint32_t)lit;
+        }
+        if (ip >= n) break;                                        // the stream ends after literals
+        if (n - ip < 2) { status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; break; }
+        const uint32_t dist = (uint32_t)__ldg(src + ip) | ((uint32_t)__ldg(src + ip + 1) << 8);
+        ip += 2;
+        if (dist == 0) { status = LZ4B200_DEC_OFFSET_ZERO; break; }
+        uint64_t mlen = 4u + (tok & 15u);
+        if (mlen == 19) {
+            for (;;) {
+                if (ip >= n) { status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; break; }
+                const uint32_t v = __ldg(src + ip++);
+                mlen += v;
+                if (v != 255) break;
+            }
+            if (status != LZ4B200_OK) break;
+        }
+        if (dist > op && dist - op > bk.decoded_off) { status = LZ4B200_DEC_OFFSET_OUT_OF_BOUNDS; break; }
+        if (mlen > (uint64_t)(cap - op)) { status = LZ4B200_DEC_OUTPUT_TOO_SMALL; break; }
+        uint32_t m = (uint32_t)mlen;
+        if (dist > op) {                                           // the part before the block: markers
+            const uint32_t pre = min(m, dist - op), from = bk.at + op - dist;
+            for (uint32_t i = sub; i < pre; i += G) dst[op + i] = kMark | (from + i);
+            op += pre; m -= pre;
+        }
+        __syncwarp(gmask);
+        if (m) copy_match<G>(dst + op, dist, m, sub, gmask);
+        op += m;
+        if (ip >= n) { status = LZ4B200_DEC_EXPECTED_ANOTHER_BYTE; break; }   // may not end on a match
+    }
+    if (status != LZ4B200_OK || op != cap) {
+        // the block's unwritten entries become poison: the resolve kernels read every entry of the window, and an
+        // entry left as whatever the scratch held could pass for a marker naming an entry far outside it
+        for (uint32_t i = op + sub; i < cap; i += G) dst[i] = kPoison;
+        if (sub == 0) atomicOr(bad, 1u);
+    }
+}
+
+// Resolve, serial part: one CTA per piece.  The carry is filled first; then, block by block with a barrier between
+// them, each block's last min(len, 64 KiB) entries take the entry their marker names, which lies in the carry or in an
+// earlier block's last 64 KiB and is already a value or poison.  The other entries are only ever read by the copy-out,
+// which resolves them with one more lookup (entries_out_kernel).  Every entry of the window these kernels read has been
+// written: the carries here, each block's entries by marker_decode_kernel (poison past the point a failing block
+// stopped), so every marker they follow is one the decode wrote.
+__global__ void __launch_bounds__(1024) resolve_tails_kernel(const MarkBlock *blocks, const MarkPiece *pieces,
+                                                             const uint32_t *carry, uint32_t *ent)
+{
+    const MarkPiece p = pieces[blockIdx.x];
+    uint32_t *c = ent + p.base;
+    for (uint32_t i = threadIdx.x; i < kCarry; i += blockDim.x) c[i] = p.carried ? carry[i] : kPoison;
+    __syncthreads();
+    for (uint32_t b = p.blk0; b < p.blk1; b++) {
+        const MarkBlock bk = blocks[b];
+        const uint32_t t = min(bk.len, kCarry);
+        uint32_t *e = ent + bk.at + (bk.len - t);
+        for (uint32_t i = threadIdx.x; i < t; i += blockDim.x) {
+            const uint32_t v = e[i];
+            if ((v & kMark) && v != kPoison) e[i] = ent[v & ~kMark];
+        }
+        __syncthreads();
+    }
+}
+
+// Resolve, parallel part, and copy-out: every range takes its part of the window's pieces (a range lies in one
+// segment, so in at most one piece), one CTA per range at a time.  A marker left (never in a block's last 64 KiB) takes
+// the entry it names, which is resolved.  A poison byte is not written; it flags its segment as unresolved.  A range
+// that starts before the piece's first touched byte belongs to another segment, whose blocks this one's look-back
+// covers: it is skipped, so it neither flags this segment nor is written again.
+__global__ void __launch_bounds__(256) entries_out_kernel(const uint32_t *ent, const MarkPiece *pieces, uint32_t np,
+                                                          const uint64_t *start, const uint64_t *len, uint64_t content_len,
+                                                          uint8_t *out, const uint64_t *out_off, uint32_t nr,
+                                                          uint32_t *unresolved)
+{
+    for (uint32_t i = blockIdx.x; i < nr; i += gridDim.x) {
+        uint64_t s, e;
+        clip_range(start[i], len[i], content_len, s, e);
+        if (s == e) continue;
+        uint32_t lo = 0, hi = np;                                  // the first piece that ends after s
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) / 2;
+            if (pieces[mid].c1 <= s) lo = mid + 1; else hi = mid;
+        }
+        for (uint32_t q = lo; q < np && pieces[q].c0 < e; q++) {
+            const MarkPiece p = pieces[q];
+            if (s < p.t0) continue;
+            const uint64_t from = max(s, p.c0), to = min(e, p.c1);
+            if (from >= to) continue;
+            const uint32_t *src = ent + p.base + kCarry + (from - p.c0);
+            uint8_t *d = out + out_off[i] + (from - s);
+            bool poison = false;
+            for (uint64_t x = threadIdx.x; x < to - from; x += blockDim.x) {
+                uint32_t v = src[x];
+                if ((v & kMark) && v != kPoison) v = ent[v & ~kMark];
+                if (v == kPoison) poison = true;
+                else d[x] = (uint8_t)v;
+            }
+            if (poison) unresolved[p.seg] = 1u;
+        }
+    }
+}
+
+// Linked frames: the blocks the ranges touch, as a difference array over the blocks (touch[first]++,
+// touch[last + 1]--), and every range's clipped length.
+__global__ void __launch_bounds__(128) range_touch_kernel(const lz4b200_frame_index_entry *index, uint32_t nb,
+                                                          uint64_t content_len, const uint64_t *start,
+                                                          const uint64_t *len, uint64_t *written, uint32_t nr,
+                                                          int32_t *touch)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nr) return;
     uint64_t s, e;
     clip_range(start[i], len[i], content_len, s, e);
     written[i] = e - s;
-    if (e > s) atomicMax(end, (unsigned long long)e);
-}
-
-// Linked frames: every range takes its part of content [g0, g1), decoded at src, one CTA per range at a time.
-__global__ void __launch_bounds__(256) range_slice_kernel(const uint8_t *src, uint64_t g0, uint64_t g1,
-                                                          const uint64_t *start, const uint64_t *len, uint64_t content_len,
-                                                          uint8_t *out, const uint64_t *out_off, uint32_t nr)
-{
-    for (uint32_t i = blockIdx.x; i < nr; i += gridDim.x) {
-        uint64_t s, e;
-        clip_range(start[i], len[i], content_len, s, e);
-        const uint64_t from = max(s, g0), to = min(e, g1);
-        if (from >= to) continue;
-        uint8_t *d = out + out_off[i] + (from - s);
-        const uint8_t *p = src + (from - g0);
-        for (uint64_t x = threadIdx.x; x < to - from; x += blockDim.x) d[x] = p[x];
-    }
+    if (e == s) return;
+    atomicAdd(touch + block_at(index, nb, s), 1);
+    atomicSub(touch + block_at(index, nb, e - 1) + 1, 1);
 }
 
 }  // namespace fr

@@ -160,16 +160,17 @@ struct DecResult {
 };
 
 // out[0..len) = out[-dist ..) with LZ77 byte-serial semantics (duplicate(), duplicate_overlapping():
-// decompress.rs:11-82; offset 1 = run fill, decompress_safe.rs:311-313).
-template <int G>
-__device__ __forceinline__ void copy_match(uint8_t *dst, uint32_t dist, uint32_t len, uint32_t sub, uint32_t gmask)
+// decompress.rs:11-82; offset 1 = run fill, decompress_safe.rs:311-313).  T is uint8_t for bytes, uint32_t for the
+// range decoder's marker entries (lz4b200_frame_range.cuh).
+template <int G, typename T>
+__device__ __forceinline__ void copy_match(T *dst, uint32_t dist, uint32_t len, uint32_t sub, uint32_t gmask)
 {
-    const uint8_t *from = dst - dist;
+    const T *from = dst - dist;
     if (dist >= len) {                       // source entirely older than this match
 #if DEC_COPY_UNROLL
         uint32_t i = sub;
         for (; i + 3 * G < len; i += 4 * G) {
-            uint8_t a = from[i], b = from[i + G], c = from[i + 2 * G], d = from[i + 3 * G];
+            T a = from[i], b = from[i + G], c = from[i + 2 * G], d = from[i + 3 * G];
             dst[i] = a; dst[i + G] = b; dst[i + 2 * G] = c; dst[i + 3 * G] = d;
         }
         for (; i < len; i += G) dst[i] = from[i];

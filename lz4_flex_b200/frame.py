@@ -455,8 +455,9 @@ def decompress_ranges_device(d_in, index: FrameIndex, starts, lengths, out=None,
     """Content bytes [starts[i], starts[i] + lengths[i]) of the frame `index` describes, for every i, decoded from the
     device tensor d_in in one call (lz4b200_frame_decompress_ranges_device).  Ranges are clipped to index.content_len
     like Python slices.  Range i goes to out[out_offsets[i]:]; with out=None the ranges are laid back to back (lengths
-    are read on the host to size `out`).  Only the blocks a range touches are decoded (a linked frame decodes from its
-    first block).  Returns (out, out_offsets, written): CUDA int64 tensors, written[i] the clipped length of range i.
+    are read on the host to size `out`).  Only the blocks a range touches are decoded; a linked frame's ranges decode
+    from a look-back of earlier blocks, doubled while a requested byte still copies content before it.  Returns (out,
+    out_offsets, written): CUDA int64 tensors, written[i] the clipped length of range i.
     Raises InvalidArgument for an index that does not fit the bytes, and DecompressionError when a block does not decode
     to its indexed length."""
     import torch
