@@ -548,9 +548,54 @@ lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const ui
                                                       const uint64_t *d_out_off, uint64_t *d_written, size_t nranges,
                                                       void *stream);
 
-/* Block decodes the context's last lz4b200_frame_decompress_ranges_device call ran: for a linked frame every block of
- * every round, look-back included; for independent blocks the (range, block) items.  0 after a call that decoded
- * nothing.  A diagnostic: it shows how far random access into a frame reached back. */
+/* Indexes many frames in DEVICE memory in one call.  Frame f is the frame that starts at d_in + d_frame_off[f], in a
+ * region of d_frame_len[f] bytes, as in lz4b200_frame_decompress_batch_device.
+ *   - with d_index NULL the call only walks the chains: *total_entries receives the sum of the blocks each chain
+ *     records, the count to allocate by.
+ *   - otherwise d_entry_off[f] receives the exclusive scan of those per-frame counts, and d_info[f] and
+ *     d_index[d_entry_off[f], + d_info[f].nblocks) receive exactly what lz4b200_frame_index_device writes to *info and
+ *     d_index for region f (payload offsets stay relative to the frame's first byte).  With max_entries below the count
+ *     the call returns INVALID_ARGUMENT having written only *total_entries.
+ *   - a frame's own error goes into its d_info[f].result and affects no other frame.
+ * The frames are walked, checksummed and sized together, in passes of whole frames whose per-block scratch fits the
+ * frame budget; a frame that alone passes the budget goes through lz4b200_frame_index_device.  Host synchronisations:
+ * one per pass kind (count, fill), plus that fallback's.  INVALID_ARGUMENT, before anything is enqueued: a null ctx or
+ * total_entries, a null d_in, d_frame_off or d_frame_len with nframes > 0, a null d_entry_off or d_info with d_index,
+ * nframes > UINT32_MAX; nframes == 0 does nothing.  d_info, d_index and d_entry_off are device memory, total_entries a
+ * host pointer.  Work runs on `stream`, which the call synchronises. */
+lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_frame_off,
+                                                const uint64_t *d_frame_len, size_t nframes,
+                                                lz4b200_frame_index_entry *d_index, size_t max_entries,
+                                                size_t *total_entries, uint64_t *d_entry_off,
+                                                lz4b200_frame_index_info *d_info, void *stream);
+
+/* Decodes byte ranges of many indexed frames in one call.  Range i reads frame f = d_range_frame[i]: d_written[i] and
+ * d_out[d_out_off[i], + d_written[i]) are what lz4b200_frame_decompress_ranges_device gives for (d_in + d_frame_off[f],
+ * d_frame_len[f], &d_info[f], d_index + d_entry_off[f], d_start[i], d_len[i]): clipped to that frame's content_len
+ * like a Python slice.  Nothing else of d_out is written.  Independent and linked frames, and frames of different block
+ * sizes, may be mixed; partial-block scratch is sized by the largest block size among the frames, so mixing 4 MiB with
+ * 64 KiB blocks makes the independent frames' windows smaller.  Linked frames share the look-back rounds; a look-back
+ * never reaches before its frame's block 0 and segments never merge across frames.
+ *   - the index is untrusted: INVALID_ARGUMENT when a frame's info fails the one-frame call's info checks, when its
+ *     entries fail that call's entry checks against its own region, when an entry span [d_entry_off[f], + nblocks) runs
+ *     past nentries, or when a range's frame id is >= nframes.  All of this is decided before any range decodes, so d_out
+ *     is then untouched.
+ *   - a block that does not decode to its indexed length is FRAME_DECOMPRESSION_ERROR for the call.
+ * Host synchronisations do not grow with the frame count: the check, one per chunk of 65 536 ranges of independent
+ * frames, one per look-back round of the linked frames, and the decode check.  lz4b200_ctx_last_range_blocks reports
+ * the call's block decodes.  INVALID_ARGUMENT, before anything is enqueued: a null ctx, a null frame array with
+ * nframes > 0, a null d_index with nentries > 0, a null range array with nranges > 0, nframes or nranges > UINT32_MAX,
+ * nentries >= UINT32_MAX, and nranges > 0 with nframes == 0.  nranges == 0 does nothing.  Every array is device memory.
+ * Work runs on `stream`, which the call synchronises. */
+lz4b200_status lz4b200_frame_decompress_ranges_batch_device(
+    lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len, size_t nframes,
+    const lz4b200_frame_index_info *d_info, const lz4b200_frame_index_entry *d_index, const uint64_t *d_entry_off,
+    size_t nentries, const uint32_t *d_range_frame, const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+    const uint64_t *d_out_off, uint64_t *d_written, size_t nranges, void *stream);
+
+/* Block decodes the context's last lz4b200_frame_decompress_ranges_device or _ranges_batch_device call ran: for a
+ * linked frame every block of every round, look-back included; for independent blocks the (range, block) items.  0
+ * after a call that decoded nothing.  A diagnostic: it shows how far random access into a frame reached back. */
 uint64_t lz4b200_ctx_last_range_blocks(const lz4b200_ctx *ctx);
 
 /* d_bound[f] = what lz4b200_frame_decoded_bound gives for region f when it holds one frame (the first frame's bound

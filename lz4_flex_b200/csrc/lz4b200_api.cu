@@ -491,26 +491,6 @@ __global__ void __launch_bounds__(128) frame_batch_tail_kernel(uint8_t *out, con
     if (f == n - 1) frame_off[n] = o;
 }
 
-// ---- the frame decoders' group pipeline ---------------------------------------------------------------------------------
-// Every frame decoder decodes a frame group by group through the same kernels: arguments, decode, resolve, gather,
-// content hash, digest (decode_group).  A group holds the blocks of one or more frames, described by one GroupFrame
-// each: the batch decoder's record walk fills one per frame, the group loop (decode_frame_blocks) one per group of a
-// frame.  Blocks are indexed frame after frame, the blocks of independent frames first and those of linked frames
-// after them.
-struct GroupFrame {
-    uint64_t in_off;                  // the frame's first byte is at src + in_off (unsigned: payload offsets add to it)
-    uint64_t out_off, out_cap;        // the group's output goes to out + out_off, at most out_cap bytes
-    uint64_t delivered;               // the frame's bytes that earlier groups delivered
-    const fw::FrameWalk *walk;        // the frame's walk
-    lz4b200_xxh32_state *content;     // the frame's content hash, carried from group to group (null: hashed by the host)
-    lz4b200_frame_result *result;
-    uint32_t base, nblocks;           // the group's descriptors of this frame: [base, base + nblocks)
-    uint32_t bad;                     // the first of them not delivered: the first to fail its checksum (kNoBlock: none),
-                                      // lowered by the resolve step to the first that fails to decode
-    uint8_t window;                   // 1: descriptor `base` is a linked window's stored pseudo-block, not output
-    uint8_t last;                     // the group ends the frame: the walk status and the EndMark rules apply
-};
-
 // ---- batch frame decoder (lz4b200_frame_decompress_batch_device) --------------------------------------------------------
 // Many independent frames per call.  Frame f is the one that starts at in + frame_off[f] in a region of frame_len[f]
 // bytes.  The host plans groups of whole frames from a count walk; each group's frames are each one group of the
@@ -552,7 +532,8 @@ __global__ void __launch_bounds__(128) frame_bound_kernel(const uint8_t *in, con
 }
 
 // Record walk of the group's frames [f0, f0 + gn), one thread per frame: each frame's descriptors at its base (from the
-// scans of the two block-count classes), its block's frame, and its GroupFrame as one group ending the frame.
+// scans of the two block-count classes), its block's frame, and its GroupFrame as one group ending the frame.  The frame
+// index passes no output (frame_out_off, frame_out_cap null: output at 0, unbounded) and no content hash (states null).
 __global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, const uint64_t *frame_off,
                                                            const uint64_t *frame_len, const uint64_t *frame_out_off,
                                                            const uint64_t *frame_out_cap, uint32_t f0, uint32_t gn,
@@ -572,10 +553,10 @@ __global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, co
     for (uint32_t k = 0; k < nb; k++) bframe[base + k] = g;
     GroupFrame p{};
     p.in_off = frame_off[f];
-    p.out_off = frame_out_off[f];
-    p.out_cap = frame_out_cap[f];
+    p.out_off = frame_out_off ? frame_out_off[f] : 0ull;
+    p.out_cap = frame_out_cap ? frame_out_cap[f] : ~0ull;
     p.walk = walks + f;
-    p.content = states + g;
+    p.content = states ? states + g : nullptr;
     p.result = results + f;
     p.base = base;
     p.nblocks = nb;
@@ -883,6 +864,11 @@ struct lz4b200_ctx {
     DevBuf<uint32_t> d_rent, d_rcarry, d_rflag;
     DevBuf<fr::MarkBlock> d_rblk;
     DevBuf<fr::MarkPiece> d_rpiece;
+    // range and index calls of one frame run as calls of many: the frame's region and entry offset, and its info; the
+    // range call's check summary
+    DevBuf<uint64_t> d_rone;
+    DevBuf<lz4b200_frame_index_info> d_iinfo;
+    DevBuf<uint32_t> d_rsum;
     uint64_t last_range_blocks = 0;           // block decodes of the last ranges call (lz4b200_ctx_last_range_blocks)
 
     bool check(cudaError_t e, const char *what)
@@ -2800,6 +2786,30 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
     return (lz4b200_status)r.status;
 }
 
+// The record walk and block checksums of the batch's frames [f0, f0 + gn), whose nb blocks were counted by
+// frame_count_kernel into ctx->d_fwalk, d_fcount and d_fnb: descriptors at ctx->d_desc, each block's frame at
+// ctx->d_bframe, one GroupFrame per frame at ctx->d_gframe, all enqueued on s.
+lz4b200_status record_frames(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off,
+                             const uint64_t *d_frame_len, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                             lz4b200_xxh32_state *states, lz4b200_frame_result *d_results, uint32_t nframes,
+                             uint32_t f0, uint32_t gn, uint32_t nb)
+{
+    CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_gframe.reserve(gn));
+    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb));
+    uint64_t *scan_ind = ctx->d_fscan.p, *scan_lnk = ctx->d_fscan.p + gn + 1;
+
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + f0, scan_ind, gn);
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + nframes + f0, scan_lnk, gn);
+    frame_record_kernel<<<(gn + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, f0, gn,
+                                                         ctx->d_fwalk.p, ctx->d_fcount.p, scan_ind, scan_lnk,
+                                                         ctx->d_desc.p, ctx->d_bframe.p, states, d_results,
+                                                         ctx->d_gframe.p);
+    if (nb) frame_batch_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, nb,
+                                                                        ctx->d_gframe.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
 // A group of the batch: frames [f0, f0 + gn), each of which the group loop decodes as one group, with nind blocks of
 // independent frames and nlnk of linked frames whose slots take `slots` bytes.  Record walk and block checksums, then
 // the group pipeline, all enqueued on s.
@@ -2809,20 +2819,10 @@ lz4b200_status decode_frame_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_
                                   uint32_t f0, uint32_t gn, uint32_t nind, uint32_t nlnk, uint64_t slots)
 {
     const uint32_t nb = nind + nlnk;
-    CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_gframe.reserve(gn));
     CTX_CUDA(ctx, ctx->d_content.reserve(gn));
-    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb));
-    uint64_t *scan_ind = ctx->d_fscan.p, *scan_lnk = ctx->d_fscan.p + gn + 1;
-
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + f0, scan_ind, gn);
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + nframes + f0, scan_lnk, gn);
-    frame_record_kernel<<<(gn + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, f0, gn,
-                                                         ctx->d_fwalk.p, ctx->d_fcount.p, scan_ind, scan_lnk,
-                                                         ctx->d_desc.p, ctx->d_bframe.p, ctx->d_content.p, d_results,
-                                                         ctx->d_gframe.p);
-    if (nb) frame_batch_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, nb,
-                                                                        ctx->d_gframe.p);
-    CTX_CUDA(ctx, cudaGetLastError());
+    const lz4b200_status st = record_frames(ctx, s, d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap,
+                                            ctx->d_content.p, d_results, nframes, f0, gn, nb);
+    if (st != LZ4B200_OK) return st;
     return decode_group(ctx, s, d_in, d_out, gn, nb, nind, slots);
 }
 
@@ -2984,8 +2984,45 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
 }
 
 // ---- frame index and range decode (no lz4_flex counterpart) ------------------------------------------------------------
-// The index: the one-frame device walk and block checksums, one sizing thread per block, then the frame decoders' own
-// result step (frame_resolve_kernel) over the sizes, so the index decides its result by the rules the decoders use.
+namespace {
+
+// The index after the walk, shared by the one-frame and the batch call: the gn frames at ctx->d_gframe, whose nb blocks
+// are described at ctx->d_desc and ctx->d_bframe (each frame's bad: its first block that fails its checksum).  One
+// sizing thread per block, the linked frames' reach check, then the frame decoders' own result step (each frame one
+// group that ends it, output at 0 and unbounded), so the index decides its results by the rules the decoders use.
+// Block k of frame g goes to index[entry_off[g] + k] (entry_off null: index[k]) and its info to info[g].  Everything is
+// enqueued on s.
+lz4b200_status index_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, uint32_t gn, uint32_t nb,
+                           const uint64_t *entry_off, lz4b200_frame_index_entry *index, lz4b200_frame_index_info *info)
+{
+    const uint32_t grid = (nb + 127) / 128, fgrid = (gn + 3) / 4;
+    CTX_CUDA(ctx, ctx->d_fhash.reserve(gn)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_reach.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    GroupFrame *frames = ctx->d_gframe.p;
+    if (nb) fr::block_size_kernel<<<grid, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, frames, nb, ctx->d_out_len.p,
+                                                       ctx->d_status.p, ctx->d_expected.p, ctx->d_out_cap.p,
+                                                       ctx->d_reach.p);
+    fr::frame_reach_kernel<<<fgrid, 128, 0, s>>>(frames, gn, ctx->d_reach.p, ctx->d_status.p, ctx->d_expected.p,
+                                                 ctx->d_out_len.p);
+    frame_resolve_kernel<<<fgrid, 128, 0, s>>>(frames, gn, ctx->d_desc.p, ctx->d_out_len.p, ctx->d_status.p,
+                                               ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_gdst.p, ctx->d_glen.p,
+                                               ctx->d_fhash.p);
+    if (nb) fr::index_entries_kernel<<<grid, 128, 0, s>>>(ctx->d_desc.p, ctx->d_bframe.p, frames, ctx->d_gdst.p,
+                                                          ctx->d_glen.p, nb, entry_off, index);
+    fr::index_info_kernel<<<(gn + 127) / 128, 128, 0, s>>>(frames, gn, info);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+// Device scratch a batch index pass takes per block (descriptor, frame, sizing results, gather offset and length) and
+// per frame (GroupFrame, result, scans, hash flag), rounded up.
+constexpr uint64_t kIndexBlockBytes = 64, kIndexFrameBytes = 256;
+
+}  // namespace
+
+// The index: the one-frame device walk and block checksums, then index_group over the frame as a group of one.
 lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
                                           lz4b200_frame_index_entry *d_index, size_t max_blocks, size_t *nblocks,
                                           lz4b200_frame_index_info *info, void *stream)
@@ -3006,23 +3043,14 @@ lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in,
     *nblocks = blocks.size();
     if (!d_index) return LZ4B200_OK;
     if (max_blocks < blocks.size() || blocks.size() >= 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
-    const uint32_t nb = (uint32_t)blocks.size(), grid = (nb + 127) / 128;
+    const uint32_t nb = (uint32_t)blocks.size();
     CTX_CUDA(ctx, ctx->d_walk.reserve(1)); CTX_CUDA(ctx, ctx->d_gframe.reserve(1)); CTX_CUDA(ctx, ctx->d_result.reserve(1));
-    CTX_CUDA(ctx, ctx->d_fhash.reserve(1)); CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_reach.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb + 1)); CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_iinfo.reserve(1));
+    CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb));
     CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_walk.p, &w, sizeof w, cudaMemcpyHostToDevice, s));
     if (nb) {
         CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_desc.p, blocks.data(), nb * sizeof(fw::FrameBlockDesc), cudaMemcpyHostToDevice, s));
-        fr::block_size_kernel<<<grid, 128, 0, s>>>(d_in, ctx->d_desc.p, nb, w.bs, w.linked != 0, ctx->d_out_len.p,
-                                                   ctx->d_status.p, ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_reach.p);
-        if (w.linked) {
-            scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_out_len.p, ctx->d_out_off.p, nb);
-            fr::block_reach_kernel<<<grid, 128, 0, s>>>(ctx->d_out_off.p, ctx->d_reach.p, nb, ctx->d_status.p,
-                                                        ctx->d_expected.p, ctx->d_out_len.p);
-        }
-        CTX_CUDA(ctx, cudaGetLastError());
+        CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bframe.p, 0, nb * sizeof(uint32_t), s));
     }
     GroupFrame p{};
     p.out_cap = ~0ull;                                        // a sufficient cap
@@ -3032,21 +3060,93 @@ lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in,
     p.bad = fw::kNoBlock;
     p.last = 1;
     CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_gframe.p, &p, sizeof p, cudaMemcpyHostToDevice, s));
-    frame_resolve_kernel<<<1, 128, 0, s>>>(ctx->d_gframe.p, 1, ctx->d_desc.p, ctx->d_out_len.p, ctx->d_status.p,
-                                           ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_gdst.p, ctx->d_glen.p, ctx->d_fhash.p);
-    if (nb) fr::index_entries_kernel<<<grid, 128, 0, s>>>(ctx->d_desc.p, ctx->d_gdst.p, ctx->d_glen.p, nb, d_index);
-    CTX_CUDA(ctx, cudaGetLastError());
-    lz4b200_frame_result r;
-    uint32_t failed = fw::kNoBlock;
-    CTX_CUDA(ctx, cudaMemcpyAsync(&r, ctx->d_result.p, sizeof r, cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaMemcpyAsync(&failed, &ctx->d_gframe.p->bad, sizeof failed, cudaMemcpyDeviceToHost, s));
+    st = index_group(ctx, s, d_in, 1, nb, nullptr, d_index, ctx->d_iinfo.p);
+    if (st != LZ4B200_OK) return st;
+    CTX_CUDA(ctx, cudaMemcpyAsync(info, ctx->d_iinfo.p, sizeof *info, cudaMemcpyDeviceToHost, s));
     CTX_CUDA(ctx, cudaStreamSynchronize(s));
-    *info = lz4b200_frame_index_info{};
-    info->block_size = w.bs;
-    info->nblocks = std::min(nb, failed);
-    info->content_len = r.written;
-    info->linked = w.linked;
-    info->result = r;
+    return LZ4B200_OK;
+}
+
+// Many frames: the batch decoder's count walk, one thread per frame, and one readback of the counts; then passes of
+// whole frames whose per-block scratch fits the frame budget, each the batch decoder's record walk and block checksums
+// and index_group, enqueued back to back.  A frame whose blocks alone pass the budget goes through the one-frame call.
+lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_frame_off,
+                                                const uint64_t *d_frame_len, size_t nframes,
+                                                lz4b200_frame_index_entry *d_index, size_t max_entries,
+                                                size_t *total_entries, uint64_t *d_entry_off,
+                                                lz4b200_frame_index_info *d_info, void *stream)
+{
+    if (!ctx || !total_entries || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_frame_off || !d_frame_len)) return LZ4B200_INVALID_ARGUMENT;
+    if (d_index && (!d_entry_off || !d_info)) return LZ4B200_INVALID_ARGUMENT;
+    *total_entries = 0;
+    if (!nframes) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t n = (uint32_t)nframes;
+    CTX_CUDA(ctx, ctx->d_fwalk.reserve(n)); CTX_CUDA(ctx, ctx->d_fcount.reserve(n));
+    CTX_CUDA(ctx, ctx->d_fnb.reserve(2 * (size_t)n));
+    frame_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ctx->frame_budget,
+                                                       ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_fnb.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    std::vector<fw::FrameCount> counts(n);
+    CTX_CUDA(ctx, cudaMemcpyAsync(counts.data(), ctx->d_fcount.p, n * sizeof(fw::FrameCount), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    std::vector<uint64_t> eoff(n);                            // the exclusive scan of the counts
+    uint64_t total = 0;
+    for (uint32_t f = 0; f < n; f++) { eoff[f] = total; total += counts[f].nblocks; }
+    *total_entries = total;
+    if (!d_index) return LZ4B200_OK;
+    if (max_entries < total) return LZ4B200_INVALID_ARGUMENT;
+    CTX_CUDA(ctx, cudaMemcpyAsync(d_entry_off, eoff.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    CTX_CUDA(ctx, ctx->d_result.reserve(n));
+    const uint64_t budget = std::min<uint64_t>(ctx->frame_budget, 1ull << 36);   // a pass indexes its blocks in 32 bits
+    std::vector<uint32_t> solo;
+    uint32_t g0 = 0;                                          // the open pass is frames [g0, f), with nb blocks
+    uint64_t nb = 0;
+    auto flush = [&](uint32_t f) {
+        lz4b200_status st = LZ4B200_OK;
+        if (f > g0) {
+            st = record_frames(ctx, s, d_in, d_frame_off, d_frame_len, nullptr, nullptr, nullptr, ctx->d_result.p, n, g0,
+                               f - g0, (uint32_t)nb);
+            if (st == LZ4B200_OK)
+                st = index_group(ctx, s, d_in, f - g0, (uint32_t)nb, d_entry_off + g0, d_index, d_info + g0);
+        }
+        g0 = f; nb = 0;
+        return st;
+    };
+    for (uint32_t f = 0; f < n; f++) {
+        const uint64_t k = counts[f].nblocks;
+        if (k * kIndexBlockBytes + kIndexFrameBytes > budget) {   // alone past the budget: the one-frame call
+            const lz4b200_status st = flush(f);
+            if (st != LZ4B200_OK) return st;
+            solo.push_back(f);
+            g0 = f + 1;
+            continue;
+        }
+        if ((nb + k) * kIndexBlockBytes + (f - g0 + 1) * kIndexFrameBytes > budget) {
+            const lz4b200_status st = flush(f);
+            if (st != LZ4B200_OK) return st;
+        }
+        nb += k;
+    }
+    lz4b200_status st = flush(n);
+    if (st != LZ4B200_OK) return st;
+    if (!solo.empty()) {
+        std::vector<uint64_t> off(n), len(n);
+        CTX_CUDA(ctx, cudaMemcpyAsync(off.data(), d_frame_off, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaMemcpyAsync(len.data(), d_frame_len, n * 8ull, cudaMemcpyDeviceToHost, s));
+        CTX_CUDA(ctx, cudaStreamSynchronize(s));
+        for (const uint32_t f : solo) {
+            size_t got = 0;
+            lz4b200_frame_index_info info;
+            st = lz4b200_frame_index_device(ctx, d_in + off[f], len[f], d_index + eoff[f], counts[f].nblocks, &got,
+                                            &info, stream);
+            if (st != LZ4B200_OK) return st;
+            CTX_CUDA(ctx, cudaMemcpyAsync(d_info + f, &info, sizeof info, cudaMemcpyHostToDevice, s));
+        }
+    }
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
     return LZ4B200_OK;
 }
 
@@ -3055,15 +3155,28 @@ namespace {
 constexpr uint32_t kRangeChunk = 65536;                      // ranges planned per launch
 constexpr uint32_t kRangeItems = 65536;                      // (range, block) items per decode launch, at most
 
+// A range call over nf indexed frames (the one-frame call is one of one frame): the frames and the ranges, all device
+// memory.  The entries are index[0, nentries).
+struct RangeCall {
+    const uint8_t *in;
+    fr::RangeFrames fr;
+    const uint64_t *frame_len;
+    uint32_t nf;
+    const lz4b200_frame_index_entry *index;
+    uint32_t nentries;
+    const uint64_t *start, *len;
+    uint8_t *out;
+    const uint64_t *out_off;
+    uint64_t *written;
+    uint32_t nr;
+};
+
 // Independent blocks: per chunk of ranges, a plan (first block, block count, item offsets) and one readback of the item
-// count; then windows of items whose partial-block slots fit the frame budget, each decoded, checked and copied.
-lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in,
-                                         const lz4b200_frame_index_info &info, const lz4b200_frame_index_entry *d_index,
-                                         const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
-                                         const uint64_t *d_out_off, uint64_t *d_written, uint32_t nr)
+// count; then windows of items whose partial-block slots (of the largest block size bs among the frames) fit the frame
+// budget, each decoded, checked and copied.
+lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const RangeCall &c, uint64_t bs)
 {
-    const uint32_t nb = (uint32_t)info.nblocks;
-    const uint64_t slot = fw::slot_bytes(info.block_size);
+    const uint64_t slot = fw::slot_bytes(bs);
     const uint32_t K = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(kRangeItems, ctx->frame_budget / std::max<uint64_t>(slot, 1)));
     CTX_CUDA(ctx, ctx->d_rfirst.reserve(kRangeChunk)); CTX_CUDA(ctx, ctx->d_rcount.reserve(kRangeChunk));
     CTX_CUDA(ctx, ctx->d_ritem.reserve(kRangeChunk + 1));
@@ -3072,14 +3185,14 @@ lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const
     CTX_CUDA(ctx, ctx->d_out_cap.reserve(K)); CTX_CUDA(ctx, ctx->d_rwant.reserve(K)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(K));
     CTX_CUDA(ctx, ctx->d_off_b.reserve(K)); CTX_CUDA(ctx, ctx->d_gdst.reserve(K)); CTX_CUDA(ctx, ctx->d_glen.reserve(K));
     CTX_CUDA(ctx, ctx->d_pick.reserve(K)); CTX_CUDA(ctx, ctx->d_out_len.reserve(K)); CTX_CUDA(ctx, ctx->d_status.reserve(K));
-    fr::RangeItems a{d_index, info.content_len, d_start, d_len, d_out_off, 0, 0, ctx->d_rfirst.p, ctx->d_ritem.p,
-                     (uint64_t)(uintptr_t)ctx->d_slots.p - (uint64_t)(uintptr_t)d_out, slot,
+    fr::RangeItems a{c.index, c.fr, c.start, c.len, c.out_off, 0, 0, ctx->d_rfirst.p, ctx->d_ritem.p,
+                     (uint64_t)(uintptr_t)ctx->d_slots.p - (uint64_t)(uintptr_t)c.out, slot,
                      ctx->d_in_off.p, ctx->d_out_off.p, ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_rwant.p,
                      ctx->d_seg_off.p, ctx->d_off_b.p, ctx->d_gdst.p, ctx->d_glen.p, ctx->d_pick.p};
-    for (uint32_t r0 = 0; r0 < nr; r0 += kRangeChunk) {
-        const uint32_t rc = std::min(kRangeChunk, nr - r0);
-        fr::range_plan_kernel<<<(rc + 127) / 128, 128, 0, s>>>(d_index, nb, info.content_len, d_start, d_len, d_written,
-                                                               r0, rc, ctx->d_rfirst.p, ctx->d_rcount.p);
+    for (uint32_t r0 = 0; r0 < c.nr; r0 += kRangeChunk) {
+        const uint32_t rc = std::min(kRangeChunk, c.nr - r0);
+        fr::range_plan_kernel<<<(rc + 127) / 128, 128, 0, s>>>(c.index, c.fr, c.start, c.len, c.written, r0, rc,
+                                                               ctx->d_rfirst.p, ctx->d_rcount.p);
         scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_rcount.p, ctx->d_ritem.p, rc);
         CTX_CUDA(ctx, cudaGetLastError());
         uint64_t total = 0;
@@ -3092,13 +3205,13 @@ lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const
             const uint32_t k = (uint32_t)std::min<uint64_t>(K, total - j0), grid = (k + 127) / 128;
             fr::range_items_kernel<<<grid, 128, 0, s>>>(a, j0, k);
             CTX_CUDA(ctx, cudaGetLastError());
-            BatchArgs b{d_in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, d_out, ctx->d_out_off.p, ctx->d_out_cap.p,
+            BatchArgs b{c.in, ctx->d_in_off.p, ctx->d_in_len.p, nullptr, c.out, ctx->d_out_off.p, ctx->d_out_cap.p,
                         ctx->d_out_len.p, ctx->d_status.p, nullptr, k, nullptr};
             const lz4b200_status st = launch_decompress(ctx, b, s);
             if (st != LZ4B200_OK) return st;
             fr::range_check_kernel<<<grid, 128, 0, s>>>(ctx->d_rwant.p, ctx->d_out_len.p, ctx->d_status.p, k, ctx->d_bad.p);
-            GatherArgs g{ctx->d_slots.p, d_in, ctx->d_seg_off.p, ctx->d_off_b.p, ctx->d_glen.p, ctx->d_glen.p,
-                         ctx->d_pick.p, nullptr, d_out, ctx->d_gdst.p, k};
+            GatherArgs g{ctx->d_slots.p, c.in, ctx->d_seg_off.p, ctx->d_off_b.p, ctx->d_glen.p, ctx->d_glen.p,
+                         ctx->d_pick.p, nullptr, c.out, ctx->d_gdst.p, k};
             gather_segments_kernel<<<std::min<uint32_t>(k, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
             CTX_CUDA(ctx, cudaGetLastError());
         }
@@ -3106,64 +3219,74 @@ lz4b200_status decode_ranges_independent(lz4b200_ctx *ctx, cudaStream_t s, const
     return LZ4B200_OK;
 }
 
-// Linked blocks: segments of consecutive touched blocks, each with a look-back of the blocks that hold the 64 KiB of
-// content before it.  A round marker-decodes every active segment's blocks (look-back included) in windows of entries
-// that fit the frame budget, resolves them and copies the ranges out; a segment with a requested byte still unresolved
-// doubles its look-back (in blocks) for the next round, and segments whose look-backs meet merge.  A segment that starts
-// at block 0 always resolves: a byte that copies content before byte 0 fails its block.
+// Linked blocks: segments of consecutive touched blocks of one frame, each with a look-back of the blocks that hold the
+// 64 KiB of content before it.  A round marker-decodes every active segment's blocks (look-back included) in windows of
+// entries that fit the frame budget, resolves them and copies the ranges out; a segment with a requested byte still
+// unresolved doubles its look-back (in blocks) for the next round, never past its frame's block 0, and segments of the
+// same frame whose look-backs meet merge.  A segment that starts at its frame's block 0 always resolves: a byte that
+// copies content before byte 0 fails its block.  The linked frames of the call share the rounds.
 struct LinkedSeg {
-    uint32_t j, a, b;                         // decoded blocks [j, b]; the ranges touch blocks [a, b]
+    uint32_t j, a, b;                         // entries: decoded blocks [j, b]; the ranges touch blocks [a, b]
+    uint32_t f;                               // the frame
 };
 
-lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in,
-                                    const lz4b200_frame_index_info &info, const lz4b200_frame_index_entry *d_index,
-                                    const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
-                                    const uint64_t *d_out_off, uint64_t *d_written, uint32_t nr)
+lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const RangeCall &c, uint64_t bs)
 {
-    const uint32_t nb = (uint32_t)info.nblocks;
-    CTX_CUDA(ctx, ctx->d_rtouch.reserve(nb + 1));
-    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rtouch.p, 0, (nb + 1) * sizeof(int32_t), s));
-    fr::range_touch_kernel<<<(nr + 127) / 128, 128, 0, s>>>(d_index, nb, info.content_len, d_start, d_len, d_written, nr,
-                                                            ctx->d_rtouch.p);
+    const uint32_t ne = c.nentries, nf = c.nf;
+    CTX_CUDA(ctx, ctx->d_rtouch.reserve(ne + 1));
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rtouch.p, 0, (ne + 1) * sizeof(int32_t), s));
+    fr::range_touch_kernel<<<(c.nr + 127) / 128, 128, 0, s>>>(c.index, c.fr, c.start, c.len, c.written, c.nr,
+                                                              ctx->d_rtouch.p);
     CTX_CUDA(ctx, cudaGetLastError());
-    std::vector<int32_t> touch(nb + 1);
-    std::vector<lz4b200_frame_index_entry> ent(nb);
-    CTX_CUDA(ctx, cudaMemcpyAsync(touch.data(), ctx->d_rtouch.p, (nb + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaMemcpyAsync(ent.data(), d_index, nb * sizeof(lz4b200_frame_index_entry), cudaMemcpyDeviceToHost, s));
+    std::vector<int32_t> touch(ne + 1);
+    std::vector<lz4b200_frame_index_entry> ent(ne);
+    std::vector<lz4b200_frame_index_info> info(nf);
+    std::vector<uint64_t> eoff(nf), foff(nf);
+    CTX_CUDA(ctx, cudaMemcpyAsync(touch.data(), ctx->d_rtouch.p, (ne + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (ne) CTX_CUDA(ctx, cudaMemcpyAsync(ent.data(), c.index, ne * sizeof(lz4b200_frame_index_entry), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(info.data(), c.fr.info, nf * sizeof(lz4b200_frame_index_info), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(eoff.data(), c.fr.entry_off, nf * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(foff.data(), c.fr.frame_off, nf * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     CTX_CUDA(ctx, cudaStreamSynchronize(s));
-    // the last block whose decoded offset is at most x, as fr::block_at finds it
-    auto block_at = [&](uint64_t x) {
-        uint32_t lo = 0, hi = nb;
-        while (hi - lo > 1) {
-            const uint32_t mid = lo + (hi - lo) / 2;
-            if (ent[mid].decoded_off <= x) lo = mid; else hi = mid;
-        }
-        return lo;
-    };
+    for (uint32_t e = 1; e <= ne; e++) touch[e] += touch[e - 1];   // > 0: a range touches entry e
     std::vector<LinkedSeg> act;
-    int32_t run = 0;
-    for (uint32_t b = 0; b < nb; b++) {
-        run += touch[b];
-        if (run <= 0) continue;
-        if (!act.empty() && act.back().b + 1 == b) { act.back().b = b; continue; }
-        const uint64_t d = ent[b].decoded_off;
-        act.push_back({d > fr::kCarry ? block_at(d - fr::kCarry) : 0u, b, b});
+    for (uint32_t f = 0; f < nf; f++) {
+        if (!info[f].linked) continue;
+        const uint32_t e0 = (uint32_t)eoff[f], nb = (uint32_t)info[f].nblocks;
+        // the last block of frame f whose decoded offset is at most x, as fr::block_at finds it
+        auto block_at = [&](uint64_t x) {
+            uint32_t lo = 0, hi = nb;
+            while (hi - lo > 1) {
+                const uint32_t mid = lo + (hi - lo) / 2;
+                if (ent[e0 + mid].decoded_off <= x) lo = mid; else hi = mid;
+            }
+            return lo;
+        };
+        for (uint32_t b = e0; b < e0 + nb; b++) {
+            if (touch[b] <= 0) continue;
+            if (!act.empty() && act.back().f == f && act.back().b + 1 == b) { act.back().b = b; continue; }
+            const uint64_t d = ent[b].decoded_off;
+            act.push_back({e0 + (d > fr::kCarry ? block_at(d - fr::kCarry) : 0u), b, b, f});
+        }
     }
-    const uint64_t window = std::min<uint64_t>(std::max<uint64_t>(ctx->frame_budget / 4, fr::kCarry + info.block_size),
-                                               1u << 30);
+    const uint64_t window = std::min<uint64_t>(std::max<uint64_t>(ctx->frame_budget / 4, fr::kCarry + bs), 1u << 30);
     const uint32_t sms = (uint32_t)ctx->sm_count;
     CTX_CUDA(ctx, ctx->d_rcarry.reserve(fr::kCarry));
+    const uint64_t before = ctx->last_range_blocks;
     uint64_t decodes = 0;
-    ctx->last_range_blocks = 0;
     std::vector<fr::MarkBlock> blk;
     std::vector<fr::MarkPiece> piece;
     struct Win { uint32_t blk0, blk1, p0, p1; uint64_t entries; };
     std::vector<Win> wins;
     while (!act.empty()) {
-        std::vector<LinkedSeg> m;                                  // merge segments whose look-backs meet
+        std::vector<LinkedSeg> m;                                  // merge a frame's segments whose look-backs meet
         for (const LinkedSeg &g : act) {
-            if (!m.empty() && g.j <= m.back().b + 1) { m.back().j = std::min(m.back().j, g.j); m.back().b = g.b; }
-            else m.push_back(g);
+            if (!m.empty() && m.back().f == g.f && g.j <= m.back().b + 1) {
+                m.back().j = std::min(m.back().j, g.j);
+                m.back().b = g.b;
+            } else {
+                m.push_back(g);
+            }
         }
         act.swap(m);
         // the round's windows: each segment's blocks in order, a piece per segment and window
@@ -3172,6 +3295,7 @@ lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint
         wins.push_back({0, 0, 0, 0, 0});
         for (uint32_t g = 0; g < act.size(); g++) {
             bool carried = false;
+            const uint64_t fo = foff[act[g].f];
             for (uint32_t k = act[g].j; k <= act[g].b;) {
                 if (used && used + fr::kCarry + ent[k].decoded_len > window) {   // a new window
                     wins.back().blk1 = (uint32_t)blk.size(); wins.back().p1 = (uint32_t)piece.size();
@@ -3180,10 +3304,11 @@ lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint
                     used = 0;
                 }
                 fr::MarkPiece p{ent[k].decoded_off, ent[k].decoded_off, ent[act[g].a].decoded_off, (uint32_t)blk.size(),
-                                0, (uint32_t)used, g, carried ? 1u : 0u, 0};
+                                0, (uint32_t)used, g, carried ? 1u : 0u, act[g].f};
                 used += fr::kCarry;
                 do {
-                    blk.push_back({ent[k].payload_off, ent[k].decoded_off, ent[k].word, ent[k].decoded_len, (uint32_t)used});
+                    blk.push_back({fo + ent[k].payload_off, ent[k].decoded_off, ent[k].word, ent[k].decoded_len,
+                                   (uint32_t)used});
                     used += ent[k].decoded_len;
                     p.c1 += ent[k].decoded_len;
                     k++;
@@ -3204,13 +3329,12 @@ lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint
         CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rflag.p, 0, act.size() * sizeof(uint32_t), s));
         for (const Win &w : wins) {
             const uint32_t k = w.blk1 - w.blk0, np = w.p1 - w.p0;
-            fr::marker_decode_kernel<32><<<(k + 3) / 4, 128, 0, s>>>(d_in, ctx->d_rblk.p + w.blk0, k, ctx->d_rent.p,
+            fr::marker_decode_kernel<32><<<(k + 3) / 4, 128, 0, s>>>(c.in, ctx->d_rblk.p + w.blk0, k, ctx->d_rent.p,
                                                                     ctx->d_bad.p);
             fr::resolve_tails_kernel<<<np, 1024, 0, s>>>(ctx->d_rblk.p, ctx->d_rpiece.p + w.p0, ctx->d_rcarry.p,
                                                          ctx->d_rent.p);
-            fr::entries_out_kernel<<<std::min<uint32_t>(nr, sms * 8), 256, 0, s>>>(
-                ctx->d_rent.p, ctx->d_rpiece.p + w.p0, np, d_start, d_len, info.content_len, d_out, d_out_off, nr,
-                ctx->d_rflag.p);
+            fr::entries_out_kernel<<<std::min<uint32_t>(c.nr, sms * 8), 256, 0, s>>>(
+                ctx->d_rent.p, ctx->d_rpiece.p + w.p0, np, c.fr, c.start, c.len, c.out, c.out_off, c.nr, ctx->d_rflag.p);
             CTX_CUDA(ctx, cudaGetLastError());
             const fr::MarkPiece &last = piece[w.p1 - 1];           // a segment cut here carries its last 64 KiB on
             if (w.p1 < piece.size() && piece[w.p1].carried)
@@ -3223,23 +3347,54 @@ lz4b200_status decode_ranges_linked(lz4b200_ctx *ctx, cudaStream_t s, const uint
         CTX_CUDA(ctx, cudaMemcpyAsync(flag.data(), ctx->d_rflag.p, act.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
         CTX_CUDA(ctx, cudaStreamSynchronize(s));
-        ctx->last_range_blocks = decodes;
+        ctx->last_range_blocks = before + decodes;
         if (bad) return LZ4B200_FRAME_DECOMPRESSION_ERROR;
         m.clear();
         for (uint32_t g = 0; g < act.size(); g++) {
             if (!flag[g]) continue;
             const LinkedSeg &x = act[g];
-            if (x.j == 0) return LZ4B200_FRAME_DECOMPRESSION_ERROR;   // cannot happen: such bytes fail their block
+            const uint32_t e0 = (uint32_t)eoff[x.f];
+            if (x.j == e0) return LZ4B200_FRAME_DECOMPRESSION_ERROR;   // cannot happen: such bytes fail their block
             const uint32_t back = 2 * (x.a - x.j);
-            m.push_back({back >= x.a ? 0u : x.a - back, x.a, x.b});
+            m.push_back({back >= x.a - e0 ? e0 : x.a - back, x.a, x.b, x.f});
         }
         act.swap(m);
     }
     return LZ4B200_OK;
 }
 
+// Every range call: the infos, entries and frame ids are checked on the device and read back once with the planners'
+// summary, before anything decodes; then the independent frames' ranges, the linked frames' ranges, and one readback
+// of the decode check.
+lz4b200_status decode_ranges(lz4b200_ctx *ctx, cudaStream_t s, const RangeCall &c)
+{
+    CTX_CUDA(ctx, ctx->d_rsum.reserve(4)); CTX_CUDA(ctx, ctx->d_bad.reserve(1));
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_rsum.p, 0, 4 * sizeof(uint32_t), s));
+    const uint32_t gx = std::min<uint32_t>(c.nf, (uint32_t)ctx->sm_count * 16);   // entries per CTA row: about 256
+    const uint32_t gy = (uint32_t)std::min<uint64_t>(65535, std::max<uint64_t>(1, (c.nentries + 256ull * gx - 1) / (256ull * gx)));
+    fr::index_check_kernel<<<dim3(gx, gy), 256, 0, s>>>(c.fr, c.frame_len, c.nf, c.index, c.nentries, ctx->d_rsum.p);
+    if (c.fr.range_frame)
+        fr::range_frame_check_kernel<<<(c.nr + 127) / 128, 128, 0, s>>>(c.fr.range_frame, c.nr, c.nf, ctx->d_rsum.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    uint32_t sum[4];
+    CTX_CUDA(ctx, cudaMemcpyAsync(sum, ctx->d_rsum.p, sizeof sum, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    if (sum[0]) return LZ4B200_INVALID_ARGUMENT;
+    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bad.p, 0, 4, s));
+    lz4b200_status st = LZ4B200_OK;
+    if (sum[3] & 1u) st = decode_ranges_independent(ctx, s, c, sum[1]);
+    if (st == LZ4B200_OK && (sum[3] & 2u)) st = decode_ranges_linked(ctx, s, c, sum[2]);
+    if (st == LZ4B200_CUDA_ERROR) return st;
+    uint32_t bad = 0;
+    CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    if (st != LZ4B200_OK) return st;
+    return bad ? LZ4B200_FRAME_DECOMPRESSION_ERROR : LZ4B200_OK;
+}
+
 }  // namespace
 
+// One frame: a range call of one frame, whose region, entry offset and info go to context scratch.
 lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n,
                                                       const lz4b200_frame_index_info *info,
                                                       const lz4b200_frame_index_entry *d_index,
@@ -3259,25 +3414,35 @@ lz4b200_status lz4b200_frame_decompress_ranges_device(lz4b200_ctx *ctx, const ui
     if (!nranges) return LZ4B200_OK;
     DeviceGuard guard(ctx->device);
     cudaStream_t s = (cudaStream_t)stream;
-    const uint32_t nb = (uint32_t)nbx, nr = (uint32_t)nranges;
-    CTX_CUDA(ctx, ctx->d_bad.reserve(1));
-    CTX_CUDA(ctx, cudaMemsetAsync(ctx->d_bad.p, 0, 4, s));
-    uint32_t bad = 0;
-    if (nb) {
-        fr::index_check_kernel<<<(nb + 255) / 256, 256, 0, s>>>(d_index, nb, n, bs, info->content_len, ctx->d_bad.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-        CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
-        CTX_CUDA(ctx, cudaStreamSynchronize(s));
-        if (bad) return LZ4B200_INVALID_ARGUMENT;
-    }
-    const lz4b200_status st = info->linked
-        ? decode_ranges_linked(ctx, s, d_in, *info, d_index, d_start, d_len, d_out, d_out_off, d_written, nr)
-        : decode_ranges_independent(ctx, s, d_in, *info, d_index, d_start, d_len, d_out, d_out_off, d_written, nr);
-    if (st == LZ4B200_CUDA_ERROR) return st;
-    CTX_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_bad.p, 4, cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaStreamSynchronize(s));
-    if (st != LZ4B200_OK) return st;
-    return bad ? LZ4B200_FRAME_DECOMPRESSION_ERROR : LZ4B200_OK;
+    const uint64_t one[3] = {0, n, 0};                        // frame offset, region length, entry offset
+    CTX_CUDA(ctx, ctx->d_rone.reserve(3)); CTX_CUDA(ctx, ctx->d_iinfo.reserve(1));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_rone.p, one, sizeof one, cudaMemcpyHostToDevice, s));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_iinfo.p, info, sizeof *info, cudaMemcpyHostToDevice, s));
+    const RangeCall c{d_in, {ctx->d_rone.p, ctx->d_iinfo.p, ctx->d_rone.p + 2, nullptr}, ctx->d_rone.p + 1, 1,
+                      d_index, (uint32_t)nbx, d_start, d_len, d_out, d_out_off, d_written, (uint32_t)nranges};
+    return decode_ranges(ctx, s, c);
+}
+
+// Ranges of many indexed frames in one call: the one-frame call's planners, with each range reading its frame.
+lz4b200_status lz4b200_frame_decompress_ranges_batch_device(
+    lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len, size_t nframes,
+    const lz4b200_frame_index_info *d_info, const lz4b200_frame_index_entry *d_index, const uint64_t *d_entry_off,
+    size_t nentries, const uint32_t *d_range_frame, const uint64_t *d_start, const uint64_t *d_len, uint8_t *d_out,
+    const uint64_t *d_out_off, uint64_t *d_written, size_t nranges, void *stream)
+{
+    if (!ctx || nframes > 0xffffffffull || nentries >= 0xffffffffull || nranges > 0xffffffffull)
+        return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_frame_off || !d_frame_len || !d_info || !d_entry_off)) return LZ4B200_INVALID_ARGUMENT;
+    if (nentries && !d_index) return LZ4B200_INVALID_ARGUMENT;
+    if (nranges && (!d_range_frame || !d_start || !d_len || !d_out || !d_out_off || !d_written))
+        return LZ4B200_INVALID_ARGUMENT;
+    ctx->last_range_blocks = 0;
+    if (!nranges) return LZ4B200_OK;
+    if (!nframes) return LZ4B200_INVALID_ARGUMENT;            // every range's frame id is out of range
+    DeviceGuard guard(ctx->device);
+    const RangeCall c{d_in, {d_frame_off, d_info, d_entry_off, d_range_frame}, d_frame_len, (uint32_t)nframes, d_index,
+                      (uint32_t)nentries, d_start, d_len, d_out, d_out_off, d_written, (uint32_t)nranges};
+    return decode_ranges(ctx, (cudaStream_t)stream, c);
 }
 
 uint64_t lz4b200_ctx_last_range_blocks(const lz4b200_ctx *ctx)
@@ -3303,6 +3468,7 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
     add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
     add(ctx->d_rtouch); add(ctx->d_rent); add(ctx->d_rcarry); add(ctx->d_rflag); add(ctx->d_rblk); add(ctx->d_rpiece);
+    add(ctx->d_rone); add(ctx->d_iinfo); add(ctx->d_rsum);
     if (const Pipeline *p = ctx->pipe.get()) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
         add(p->d_tickets);

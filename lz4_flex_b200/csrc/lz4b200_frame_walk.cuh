@@ -307,4 +307,26 @@ FW_FN void frame_count(const uint8_t *in, uint64_t n, FrameWalk &w, FrameCount &
 }
 
 }  // namespace fw
+
+// ---- the frame decoders' group pipeline ---------------------------------------------------------------------------------
+// Every frame decoder decodes a frame group by group through the same kernels: arguments, decode, resolve, gather,
+// content hash, digest (decode_group in lz4b200_api.cu).  A group holds the blocks of one or more frames, described by
+// one GroupFrame each: the batch decoder's record walk fills one per frame, the group loop (decode_frame_blocks) one per
+// group of a frame.  Blocks are indexed frame after frame, the blocks of independent frames first and those of linked
+// frames after them.  The frame index (lz4b200_frame_range.cuh) sizes the blocks of such groups and runs their result
+// step.
+struct GroupFrame {
+    uint64_t in_off;                  // the frame's first byte is at src + in_off (unsigned: payload offsets add to it)
+    uint64_t out_off, out_cap;        // the group's output goes to out + out_off, at most out_cap bytes
+    uint64_t delivered;               // the frame's bytes that earlier groups delivered
+    const fw::FrameWalk *walk;        // the frame's walk
+    lz4b200_xxh32_state *content;     // the frame's content hash, carried from group to group (null: hashed by the host)
+    lz4b200_frame_result *result;
+    uint32_t base, nblocks;           // the group's descriptors of this frame: [base, base + nblocks)
+    uint32_t bad;                     // the first of them not delivered: the first to fail its checksum (kNoBlock: none),
+                                      // lowered by the resolve step to the first that fails to decode
+    uint8_t window;                   // 1: descriptor `base` is a linked window's stored pseudo-block, not output
+    uint8_t last;                     // the group ends the frame: the walk status and the EndMark rules apply
+};
+
 }  // namespace lz4b200

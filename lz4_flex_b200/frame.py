@@ -443,6 +443,11 @@ def index_frame_device(d_in, ctx: _block.Context | None = None, stream: int | No
                                       C.byref(info), s)
     if st != 0:
         raise error_from_status(st, detail=ctx.last_cuda_error())
+    return _frame_index(info, entries)
+
+
+def _frame_index(info, entries) -> FrameIndex:
+    """The FrameIndex of an lz4b200_frame_index_info and the frame's entries (at least info.nblocks rows)."""
     r = info.result
     err = None if r.status in (0, _CONTENT_CHECKSUM) else error_from_status(r.status, r.block_status, "", r.err_expected,
                                                                             r.err_actual)
@@ -491,6 +496,127 @@ def decompress_ranges_device(d_in, index: FrameIndex, starts, lengths, out=None,
         ctx.handle, d_in.data_ptr() if d_in.numel() else None, d_in.numel(), C.byref(index._info),
         index.entries.data_ptr() if index.nblocks else None, st_t.data_ptr(), ln_t.data_ptr(), out.data_ptr(),
         oo.data_ptr(), written.data_ptr(), nr, s)
+    if st == 101:
+        raise DecompressionError(ValueError("a block does not decode to its indexed length"))
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return out, oo, written
+
+
+@dataclass
+class FrameIndexes:
+    """What index_frames_device() returns for many frames, all CUDA int64 tensors: `infos` (n, 9), each row one
+    lz4b200_frame_index_info (block size, nblocks, content length, linked, then the frame's result); `entries` (total,
+    3) as in FrameIndex, frame i's at rows entry_offsets[i] onwards; and the frames' `offsets` and `lengths` in d_in."""
+    infos: "object"
+    entries: "object"
+    entry_offsets: "object"
+    offsets: "object"
+    lengths: "object"
+    _host: Optional[np.ndarray] = None
+
+    def __len__(self) -> int:
+        return self.infos.shape[0]
+
+    def _rows(self) -> np.ndarray:
+        if self._host is None:
+            self._host = np.ascontiguousarray(self.infos.cpu().numpy())
+            self._eoff = self.entry_offsets.cpu().numpy()
+        return self._host
+
+    def content_lens(self) -> np.ndarray:
+        """Every frame's content length (the decoded total of its indexed blocks), on the host."""
+        return self._rows()[:, 2].copy()
+
+    def frame(self, i: int) -> FrameIndex:
+        """Frame i's FrameIndex: what index_frame_device() returns for its region, usable with
+        decompress_ranges_device() on that region."""
+        info = _native.FrameIndexInfoC.from_buffer_copy(self._rows()[i].tobytes())
+        e0 = int(self._eoff[i])
+        return _frame_index(info, self.entries[e0:e0 + info.nblocks])
+
+
+def index_frames_device(d_in, offsets, lengths, ctx: _block.Context | None = None,
+                        stream: int | None = None) -> FrameIndexes:
+    """Indexes many frames in the device tensor d_in in one call (lz4b200_frame_index_batch_device): frame i is the one
+    that starts at d_in[offsets[i]] in a region of lengths[i] bytes, and its index is what index_frame_device() gives
+    for that region (FrameIndexes.frame).  Two calls: one counts the blocks, the other fills the index."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    offs, lens = _device_i64(offsets, dev, "offsets"), _device_i64(lengths, dev, "lengths")
+    n = offs.numel()
+    if lens.numel() != n:
+        raise ValueError("offsets and lengths differ in length")
+    infos = torch.zeros((n, 9), dtype=torch.int64, device=dev)
+    eoff = torch.zeros(n, dtype=torch.int64, device=dev)
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    L = _native.lib()
+    ptr = lambda t: t.data_ptr() if t.numel() else None
+    count = C.c_size_t(0)
+    st = L.lz4b200_frame_index_batch_device(ctx.handle, ptr(d_in), ptr(offs), ptr(lens), n, None, 0, C.byref(count),
+                                            None, None, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    entries = torch.empty((max(count.value, 1), 3), dtype=torch.int64, device=dev)
+    if n:
+        st = L.lz4b200_frame_index_batch_device(ctx.handle, ptr(d_in), ptr(offs), ptr(lens), n, entries.data_ptr(),
+                                                count.value, C.byref(count), eoff.data_ptr(), infos.data_ptr(), s)
+        if st != 0:
+            raise error_from_status(st, detail=ctx.last_cuda_error())
+    return FrameIndexes(infos, entries[:count.value], eoff, offs, lens)
+
+
+def decompress_frames_ranges_device(d_in, index: FrameIndexes, frames, starts, lengths, out=None, out_offsets=None,
+                                    ctx: _block.Context | None = None, stream: int | None = None):
+    """Content bytes [starts[i], starts[i] + lengths[i]) of frame frames[i] of `index`, for every i, decoded from the
+    device tensor d_in in one call (lz4b200_frame_decompress_ranges_batch_device).  Range i is what
+    decompress_ranges_device() gives on index.frame(frames[i]) and that frame's region: clipped to the frame's content
+    like a Python slice.  Independent and linked frames may be mixed.  Range i goes to out[out_offsets[i]:]; with
+    out=None the ranges are laid back to back (lengths and frame ids are read on the host to size `out`).  Returns
+    (out, out_offsets, written): CUDA int64 tensors, written[i] the clipped length of range i.
+    Raises ValueError for a frame id out of range or an index that does not fit the bytes, and DecompressionError when
+    a block does not decode to its indexed length."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    st_t, ln_t = _device_i64(starts, dev, "starts"), _device_i64(lengths, dev, "lengths")
+    fr_t = _device_i64(frames, dev, "frames")
+    nr, nf = st_t.numel(), len(index)
+    if ln_t.numel() != nr or fr_t.numel() != nr:
+        raise ValueError("frames, starts and lengths differ in length")
+    if (out is None) != (out_offsets is None):
+        raise ValueError("out and out_offsets go together")
+    if out is None:
+        a, b, f = _host_i64(starts, "starts"), _host_i64(lengths, "lengths"), _host_i64(frames, "frames")
+        if f.size and f.max() >= nf:
+            raise ValueError("lz4b200: invalid argument (a frame id out of range)")
+        c = index.content_lens()[f]
+        s0 = np.minimum(a, c)
+        clipped = np.minimum(b, c - s0)
+        ends = np.cumsum(clipped)
+        oo = torch.as_tensor(ends - clipped, dtype=torch.int64).to(dev)
+        out = torch.empty(max(int(ends[-1]) if nr else 0, 1), dtype=torch.uint8, device=dev)
+    else:
+        _device_u8(out, "out")
+        oo = _device_i64(out_offsets, dev, "out_offsets")
+        if oo.numel() != nr:
+            raise ValueError("out_offsets needs one entry per range")
+    # frame ids as uint32: an id outside [0, 2^32) becomes 2^32 - 1, which no call's frame count reaches
+    fr32 = torch.where((fr_t < 0) | (fr_t > 0xFFFFFFFF), torch.full_like(fr_t, 0xFFFFFFFF), fr_t).to(torch.int32)
+    written = torch.zeros(nr, dtype=torch.int64, device=dev)
+    if stream is not None:
+        torch.cuda.current_stream(dev).synchronize()                       # the tensors above were filled on torch's stream
+    ptr = lambda t: t.data_ptr() if t.numel() else None
+    st = _native.lib().lz4b200_frame_decompress_ranges_batch_device(
+        ctx.handle, ptr(d_in), ptr(index.offsets), ptr(index.lengths), nf, ptr(index.infos), ptr(index.entries),
+        ptr(index.entry_offsets), index.entries.shape[0], ptr(fr32), ptr(st_t), ptr(ln_t), out.data_ptr(), ptr(oo),
+        ptr(written), nr, s)
     if st == 101:
         raise DecompressionError(ValueError("a block does not decode to its indexed length"))
     if st != 0:
