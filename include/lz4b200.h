@@ -368,6 +368,20 @@ lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx,
     uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
     size_t nframes, void *stream);
 
+/* lz4b200_frame_compress_batch_device for BlockMode::Linked: d_out[d_frame_off[f], d_frame_off[f + 1]) holds exactly what
+ * FrameEncoder::with_frame_info(info_f, Vec::new()), write_all(in_f) and finish() write with linked blocks, where every
+ * block may match into the 64 KiB before it.  Arguments, Auto block sizes, content sizes, packing, bound and
+ * asynchrony are those of lz4b200_frame_compress_batch_device, and so is the order of argument errors, except that
+ * info->linked == 0 is INVALID_ARGUMENT where that call reports FRAME_LINKED_UNSUPPORTED.
+ * Frame f costs one serial chain: its blocks are parsed one after another by one matcher warp, because each block's
+ * parse starts from the hash table the block before it left (frame/compress.rs:261-371).  Frames run in parallel,
+ * longest first, so the call is for many linked frames at once; one large linked frame runs at the speed of one chain. */
+lz4b200_status lz4b200_frame_compress_linked_batch_device(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *in_off, const uint64_t *in_len,
+    const lz4b200_frame_info *info,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
+    size_t nframes, void *stream);
+
 /* Block-range form used for multi-GPU sharding (SURVEY.md §8e): compress frame blocks
  * [first_block, first_block + nblocks) of a stream cut into `block_size`-byte blocks.  `d_in`
  * points at the first byte of block `first_block` (device memory, `in_len` bytes for this

@@ -153,6 +153,8 @@ SIGNATURES = {
     "lz4b200_frame_compress": (_i32, [_vp, _vp, _sz, C.POINTER(FrameInfoC), _sz, _vp, _sz, _psz]),
     "lz4b200_frame_compress_device": (_i32, [_vp, _vp, _sz, C.POINTER(FrameInfoC), _sz, _vp, _sz, _vp, _vp]),
     "lz4b200_frame_compress_batch_device": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp, _sz, _vp]),
+    "lz4b200_frame_compress_linked_batch_device": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp, _sz,
+                                                           _vp]),
     "lz4b200_frame_compress_blocks_device": (_i32, [_vp, _vp, _sz, _sz, C.c_uint64, _vp, _sz, _vp, _vp, _vp]),
     "lz4b200_frame_blocks_bound": (_sz, [_sz, _sz]),
     "lz4b200_frame_range_compress": (_i32, [_vp, _vp, _sz, _sz, C.c_uint64, _vp, _vp, _vp]),

@@ -20,6 +20,7 @@
 #include "lz4b200_frame_range.cuh"
 #include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
+#include "lz4b200_enc_linked.cuh"
 #include "lz4b200_solo_kernel.cuh"
 #ifdef LZ4B200_AB_VARIANTS
 // A/B build (lz4_flex_b200/liblz4b200_ab.so, -DLZ4B200_AB_VARIANTS): the kernels that lost their measurements stay
@@ -798,6 +799,7 @@ struct lz4b200_ctx {
     int dec_ctas_per_sm = 0;
     int enc16s_ctas_per_sm = 0, enc32s_ctas_per_sm = 0;   // split (matcher+emitter) encoder
     int enc_gtab_ctas_per_sm = 0;             // global-table encoder (must reach ENC_GTAB_CTAS)
+    int enc_linked_ctas_per_sm = 0;           // linked-frame chain encoder
     int high_priority = 0;                    // lz4b200_ctx_set_priority(ctx, 1): pipeline streams get the highest priority
     DevBuf<uint16_t> d_gtab16;                // global u16 tables (lz4_compress_blocks_gtab / _gtab16)
     const uint32_t *pipe_tickets = nullptr;  // base of the host pipeline's ticket blocks (selects a table region)
@@ -854,6 +856,7 @@ struct lz4b200_ctx {
     DevBuf<uint8_t> d_fhash;
     DevBuf<GroupFrame> d_gframe;              // the frames of a decode group
     DevBuf<fb::FramePlan> d_fplan;            // batch frame encoder: the host's plan, one entry per frame
+    DevBuf<uint32_t> d_forder;                // linked batch frame encoder: the frames longest first, one per ticket
     // frame index and range decode: per block a linked block's reach; per range of a chunk its first block, block count
     // and item offset; per item of a window the length its block must decode to.  Linked frames: the touched blocks'
     // difference array, a window's marker entries, blocks and pieces, the carry from window to window, and per segment
@@ -1284,6 +1287,9 @@ lz4b200_status lz4b200_ctx_create(int device, lz4b200_ctx **out)
              ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
                             &ctx->enc32s_ctas_per_sm, lz4_compress_blocks_split<uint32_t, kEnc32Pairs, false>, kEnc32Pairs * 64,
                             split_smem_bytes<uint32_t, kEnc32Pairs>()), "occupancy enc32 split") &&
+             ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+                            &ctx->enc_linked_ctas_per_sm, lz4_compress_frames_linked, kLinkedPairs * 64,
+                            linked_smem_bytes()), "occupancy linked") &&
              ctx->check(cudaFuncSetAttribute(lz4_compress_blocks_solo2, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              (int)kSolo2SmemBytes), "solo2 smem") &&
              ctx->check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->enc_solo2_ctas_per_sm, lz4_compress_blocks_solo2, 64,
@@ -2198,9 +2204,13 @@ void frame_plan(fb::FramePlan &p, const lz4b200_frame_info &info, uint64_t in_of
 // device position d_pos_in moves every block *d_pos_in bytes further, and *d_pos_out receives the end of the blocks.
 // With `content_checksum` one CTA per frame hashes its content; with d_frame_off one thread per frame writes its
 // header, EndMark, digest (when hashed) and d_frame_off[f], and d_frame_off[n] the total.
+// With `linked_order` (a host array of n frame indices, longest frame first) the frames are BlockMode::Linked: one
+// launch of lz4_compress_frames_linked runs one chain per frame, taking frames in that order, in place of
+// launch_compress, and everything else is the same.
 lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::FramePlan *plan, uint32_t n,
                                uint32_t max_in_len, bool block_checksums, bool content_checksum, uint8_t *d_out,
-                               uint64_t *d_frame_off, const uint64_t *d_pos_in, uint64_t *d_pos_out, cudaStream_t s)
+                               uint64_t *d_frame_off, const uint64_t *d_pos_in, uint64_t *d_pos_out, cudaStream_t s,
+                               const uint32_t *linked_order = nullptr)
 {
     const fb::FramePlan &last = plan[n - 1];
     const uint32_t nb = last.first_block + (uint32_t)fb::frame_blocks(last);
@@ -2229,8 +2239,20 @@ lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::
         CTX_CUDA(ctx, cudaGetLastError());
         BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
                     ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
-        const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
-        if (st != LZ4B200_OK) return st;
+        if (linked_order) {
+            CTX_CUDA(ctx, ctx->d_forder.reserve(n));
+            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_forder.p, linked_order, n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+            const uint32_t grid = std::min<uint32_t>((n + kLinkedPairs - 1) / kLinkedPairs,
+                                                     (uint32_t)(ctx->sm_count * ctx->enc_linked_ctas_per_sm));
+            lz4_compress_frames_linked<<<grid, kLinkedPairs * 64, linked_smem_bytes(), s>>>(a, ctx->d_fplan.p,
+                                                                                           ctx->d_forder.p, n,
+                                                                                           ctx->d_tickets.p + 6);
+            ctx->last_kernel[0] = "lz4_compress_frames_linked";
+            CTX_CUDA(ctx, cudaGetLastError());
+        } else {
+            const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
+            if (st != LZ4B200_OK) return st;
+        }
         frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb,
                                                                 block_checksums ? 4u : 0u, ctx->d_info.p,
                                                                 ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
@@ -2447,18 +2469,23 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
     return LZ4B200_OK;
 }
 
-// lz4b200_frame_compress_device for each of many inputs, frames packed back to back, in one call: the host plans every
-// frame (fb::plan_frame) and compress_frames enqueues them all on `stream`.
-lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *in_off,
-                                                   const uint64_t *in_len, const lz4b200_frame_info *info,
-                                                   uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
-                                                   size_t nframes, void *stream)
+}  // extern "C"
+
+namespace {
+
+// lz4b200_frame_compress_batch_device and its linked form: the host plans every frame (fb::plan_frame) and
+// compress_frames enqueues them all on `stream`.  `linked` is the form called; the argument checks differ only in what
+// info->linked is answered with.
+lz4b200_status compress_frame_batch(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *in_off,
+                                    const uint64_t *in_len, const lz4b200_frame_info *info, uint8_t *d_out,
+                                    size_t out_cap, uint64_t *d_frame_off, size_t nframes, void *stream, bool linked)
 {
     if (!ctx || !info || !d_frame_off || (nframes && (!in_off || !in_len || !d_out))) return LZ4B200_INVALID_ARGUMENT;
     if (!d_in)
         for (size_t f = 0; f < nframes; f++)
             if (in_len[f]) return LZ4B200_INVALID_ARGUMENT;
-    if (info->linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    if (!linked && info->linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    if (linked && !info->linked) return LZ4B200_INVALID_ARGUMENT;
     const int id = info->block_size_id;
     if ((id != 0 && (id < 4 || id > 7)) || nframes > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
     const uint32_t tail = info->content_checksum ? 8u : 4u;
@@ -2491,8 +2518,38 @@ lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8
     // blocks on both sides of 64 KiB run both encoders whatever the bound says; an unknown bound (0) makes the
     // launcher's record name both
     const uint32_t max_in_len = small && max_len > 65536u ? 0u : (uint32_t)max_len;
+    std::vector<uint32_t> order;
+    if (linked) {                                           // a launch lasts as long as its longest chain: start those first
+        order.resize(nframes);
+        for (size_t f = 0; f < nframes; f++) order[f] = (uint32_t)f;
+        std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return in_len[x] > in_len[y]; });
+    }
     return compress_frames(ctx, d_in, plan.data(), (uint32_t)nframes, max_in_len, info->block_checksums,
-                           info->content_checksum, d_out, d_frame_off, nullptr, nullptr, s);
+                           info->content_checksum, d_out, d_frame_off, nullptr, nullptr, s,
+                           linked ? order.data() : nullptr);
+}
+
+}  // namespace
+
+extern "C" {
+
+// lz4b200_frame_compress_device for each of many inputs, frames packed back to back, in one call.
+lz4b200_status lz4b200_frame_compress_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *in_off,
+                                                   const uint64_t *in_len, const lz4b200_frame_info *info,
+                                                   uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
+                                                   size_t nframes, void *stream)
+{
+    return compress_frame_batch(ctx, d_in, in_off, in_len, info, d_out, out_cap, d_frame_off, nframes, stream, false);
+}
+
+// The same for BlockMode::Linked frames: one chain per frame (lz4b200_enc_linked.cuh).
+lz4b200_status lz4b200_frame_compress_linked_batch_device(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                          const uint64_t *in_off, const uint64_t *in_len,
+                                                          const lz4b200_frame_info *info, uint8_t *d_out,
+                                                          size_t out_cap, uint64_t *d_frame_off, size_t nframes,
+                                                          void *stream)
+{
+    return compress_frame_batch(ctx, d_in, in_off, in_len, info, d_out, out_cap, d_frame_off, nframes, stream, true);
 }
 
 namespace {
@@ -3466,7 +3523,7 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_status); add(ctx->d_walk); add(ctx->d_desc); add(ctx->d_bad); add(ctx->d_content); add(ctx->d_result);
     add(ctx->d_fwalk); add(ctx->d_fcount); add(ctx->d_fnb); add(ctx->d_bframe);
     add(ctx->d_bslot); add(ctx->d_glen); add(ctx->d_fscan); add(ctx->d_gdst); add(ctx->d_fhash); add(ctx->d_fplan);
-    add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
+    add(ctx->d_forder); add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
     add(ctx->d_rtouch); add(ctx->d_rent); add(ctx->d_rcarry); add(ctx->d_rflag); add(ctx->d_rblk); add(ctx->d_rpiece);
     add(ctx->d_rone); add(ctx->d_iinfo); add(ctx->d_rsum);
     if (const Pipeline *p = ctx->pipe.get()) {

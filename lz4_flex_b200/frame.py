@@ -1,4 +1,5 @@
-"""lz4_flex::frame, H100 edition (encoder: independent-block mode; decoder: independent and linked blocks).
+"""lz4_flex::frame, H100 edition (encoder: independent blocks, and linked blocks for many frames per call; decoder:
+independent and linked blocks).
 
 FrameInfo / BlockSize / BlockMode / FrameEncoder / FrameDecoder with the reference's names and behaviour
 (src/frame/header.rs:39-192, src/frame/compress.rs:62-438, src/frame/decompress.rs:48-422).  The container
@@ -11,8 +12,10 @@ device: header, EndMark and both checksums are written or verified by kernels, a
 
 BlockMode::Linked chains every block to its frame's earlier output.  The DECODER handles it on the device
 (lz4_decompress_blocks_linked: a block waits for the predecessors an offset reaches into), so frames written by
-`lz4` / LZ4F / pyarrow with their default linked blocks decode; the ENCODER refuses it (LinkedBlocksUnsupported):
-a linked encode is one serial chain per frame, which is not what a GPU batch path is for.
+`lz4` / LZ4F / pyarrow with their default linked blocks decode.  The encoders refuse it (LinkedBlocksUnsupported):
+a linked encode is one serial chain per frame, which is not what a GPU batch path is for.  The exception is many
+linked frames already in GPU memory: compress_linked_frames_device() runs one chain per frame, all frames of the call
+in parallel, and writes what lz4_flex's linked FrameEncoder writes for each.  A lone linked frame is faster on a CPU.
 """
 from __future__ import annotations
 
@@ -178,12 +181,32 @@ def compress_frames_device(d_in, offsets, lengths, frame_info: FrameInfo | None 
     itself is ignored).  The work runs on torch's current stream (or `stream`); the call returns once the total length
     has been read back.  Returns (view of `out` that holds the frames, CUDA int64 tensor of len(offsets) + 1 frame
     offsets: frame i is out[frame_offsets[i]:frame_offsets[i + 1]]).  Raises what compress_frame() raises."""
-    import torch
-    _device_u8(d_in, "d_in")
-    ctx = ctx or _block.default_context()
     info = frame_info or FrameInfo()
     if info.block_mode == BlockMode.Linked:
         raise LinkedBlocksUnsupported()
+    return _compress_frame_batch(_native.lib().lz4b200_frame_compress_batch_device, d_in, offsets, lengths, info, out,
+                                 ctx, stream)
+
+
+def compress_linked_frames_device(d_in, offsets, lengths, frame_info: FrameInfo | None = None, out=None,
+                                  ctx: _block.Context | None = None, stream: int | None = None):
+    """compress_frames_device() for BlockMode::Linked (lz4b200_frame_compress_linked_batch_device): frame i is
+    byte-identical to what lz4_flex's FrameEncoder writes for input i with linked blocks, where each block may match
+    into the 64 KiB before it.  frame_info must have block_mode=BlockMode.Linked (None: the default FrameInfo with
+    linked blocks); an independent one raises ValueError.  Arguments, return value and stream behaviour are those of
+    compress_frames_device().  Each frame is one serial chain on the GPU and frames run in parallel, so this call is
+    for many frames at once: one large frame runs at the speed of one chain (DESIGN.md §6)."""
+    info = frame_info or FrameInfo(block_mode=BlockMode.Linked)
+    if info.block_mode != BlockMode.Linked:
+        raise ValueError("compress_linked_frames_device: frame_info.block_mode must be BlockMode.Linked")
+    return _compress_frame_batch(_native.lib().lz4b200_frame_compress_linked_batch_device, d_in, offsets, lengths, info,
+                                 out, ctx, stream)
+
+
+def _compress_frame_batch(fn, d_in, offsets, lengths, info: FrameInfo, out, ctx, stream):
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
     offs, lens = _host_i64(offsets, "offsets"), _host_i64(lengths, "lengths")
     n = offs.size
     if lens.size != n:
@@ -202,9 +225,8 @@ def compress_frames_device(d_in, offsets, lengths, frame_info: FrameInfo | None 
     _device_u8(out, "out")
     s = stream if stream is not None else torch.cuda.current_stream(d_in.device).cuda_stream
     frame_offsets = torch.empty(n + 1, dtype=torch.int64, device=out.device)
-    st = _native.lib().lz4b200_frame_compress_batch_device(
-        ctx.handle, d_in.data_ptr() if d_in.numel() else None, offs.ctypes.data, lens.ctypes.data, C.byref(ci),
-        out.data_ptr() if out.numel() else None, out.numel(), frame_offsets.data_ptr(), n, s)
+    st = fn(ctx.handle, d_in.data_ptr() if d_in.numel() else None, offs.ctypes.data, lens.ctypes.data, C.byref(ci),
+            out.data_ptr() if out.numel() else None, out.numel(), frame_offsets.data_ptr(), n, s)
     if st != 0:
         raise error_from_status(st, detail=ctx.last_cuda_error())
     if stream is None:
