@@ -24,6 +24,7 @@
 // Hand-off: two halves of 16 tuples, mbarriers "full[h]" / "empty[h]" per pair in shared memory — the matcher
 // never waits unless the emitter is two batches behind.
 #pragma once
+#include <type_traits>
 #ifndef ENC_GTAB_L1
 #define ENC_GTAB_L1 0   // 1: global-table reads may hit L1 (same-SM coherent); 0: L2 only
 #endif
@@ -32,6 +33,9 @@
 #endif
 #ifndef ENC_FASTW
 #define ENC_FASTW 1     // 1: settle slot collisions of the first <= 4 probes with shuffles instead of match.any
+#endif
+#ifndef ENC_PROBE_BOUND
+#define ENC_PROBE_BOUND 0   // profile builds only (tests/dev/enc_phase_probe.py -D ENC_PROBE_BOUND=1): see kProbeBound
 #endif
 #ifndef ENC_RI_PATCH
 #define ENC_RI_PATCH 0  // 1: re-insert folded into the batch commit (no store->load dependency); 0: store + syncwarp first
@@ -367,7 +371,17 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
 {
     static_assert(!kTag || (kGT && sizeof(TabT) == 4), "tagged entries: global u32 tables");
     constexpr uint32_t kInvalid = kTag ? 0xffffffffu : TabTraits<TabT>::kInvalid;
+    // Candidate loads of a probe batch in two tiers (global-memory words only): lanes 0..3 and the rest.  Four lanes
+    // cover the hits the shuffle check below settles; on H100, 2 lanes were as fast and 8 slower (DESIGN.md §6).
+    constexpr bool kTiered = !kTag && std::is_same<View, WordView>::value;
+    constexpr uint32_t kTier1 = 4;
+#if defined(LZ4B200_ENC_PROFILE) && ENC_PROBE_BOUND
+    constexpr bool kProbeBound = kTiered;   // tier 2 loads nothing and never hits: wrong output, a bound on what tiers save
+#else
+    constexpr bool kProbeBound = false;
+#endif
     const uint32_t lt_mask = (1u << lane) - 1u;
+    const bool t1 = lane < kTier1;
 #ifdef LZ4B200_ENC_PROFILE
     EncProfile prof;
 #endif
@@ -397,6 +411,9 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
     const uint32_t last_probe = n - 12;
     const uint32_t lim = n - 6;                                 // matches end before the last END_OFFSET bytes
     uint32_t anchor = 0, cur = 0;
+    // Tier 2's candidate words (kTiered).  They live across batches and sequences, updated in place by the loads: if
+    // their registers were free after a batch that tier 1 decided, the next value put there would wait for tier 2's loads.
+    uint2 w2 = make_uint2(0u, 0u);
     bool ri = false;                                            // T[H(cur-2)] = cur-2 still owed (compress.rs:460-461)
     if (!cont) {                                                // compress.rs:353-359
         uint32_t lo, hi; view.ro5(0, lo, hi);
@@ -457,17 +474,30 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
             // for the rest.
             bool chk = live && cnd != kInvalid && p - cnd <= 65535u && tag_ok;
             bool hit;
-            if (kTag) {                                         // only lanes whose tag agrees touch memory
+            uint32_t hits;
+            if constexpr (kTag) {                               // only lanes whose tag agrees touch memory
                 uint32_t c4 = ~v4;
                 if (chk) c4 = view.ro4(cnd);
                 hit = chk & (c4 == v4);
+                hits = __ballot_sync(kFull, hit);
+            } else if constexpr (kTiered) {
+                // The first hit wins, so a batch whose first speculative hit w0 lies in lanes 0..kTier1-1 and stays
+                // exact is decided by those lanes' candidates alone.  Both tiers' loads go out now, back to back; the
+                // hit ballot waits for tier 1 only, and tier 2's registers are read only in the !exact path below.
+                // Candidates are scattered over up to 64 KiB of history, so a batch that waited for all 32 would
+                // usually wait for one that misses L2.
+                uint2 w1 = make_uint2(0u, 0u);
+                view.ro4_issue(w1, cnd, chk && t1);
+                view.ro4_issue(w2, cnd, chk && !t1 && !kProbeBound);
+                hit = chk & t1 & (view.ro4_join(w1, cnd) == v4);
+                hits = __ballot_sync(kFull, hit);
             } else {
                 hit = chk & (view.ro4(chk ? cnd : 0u) == v4);
+                hits = __ballot_sync(kFull, hit);
             }
-            uint32_t hits = __ballot_sync(kFull, hit);
             const uint32_t terms = (base + 31u * stride > last_probe) ? __ballot_sync(kFull, term) : 0u;   // uniform: only near the block's end
             ENC_PROF(phase(kPhProbe));
-            const uint32_t w0 = hits ? (uint32_t)__ffs(hits) - 1u : 32u;
+            uint32_t w0 = hits ? (uint32_t)__ffs(hits) - 1u : 32u;
             uint32_t same = 1u << lane;                         // lanes of this batch on my slot (incl. me)
             bool exact = w0 == 0u;
 #if ENC_FASTW
@@ -479,6 +509,17 @@ __device__ __forceinline__ void match_block_view(View &view, uint32_t n, TabT *t
 #endif
             if (!exact) {
                 same = __match_any_sync(kFull, key);
+                if constexpr (kTiered) {
+                    // Tier 1 has no hit, or its hit w0 sits behind a slot collision that the forwarded re-check may
+                    // resolve against it: from here on every lane's hit counts.  w0 >= kTier1 >= 4 in the first case and
+                    // unchanged in the second, so the shuffle check above has nothing to add.  `same` always holds this
+                    // lane's bit, so `mine` is ~0; reading tier 2 through it keeps the compiler from moving the read
+                    // (and its wait for the loads) above the branch.
+                    const uint32_t mine = 0u - ((same >> lane) & 1u);
+                    if (!t1 && !kProbeBound) hit = chk & (view.ro4_join(w2, cnd & mine) == v4);
+                    hits = __ballot_sync(kFull, hit);
+                    w0 = hits ? (uint32_t)__ffs(hits) - 1u : 32u;
+                }
                 const uint32_t prior = same & lt_mask;
                 const uint32_t le0 = w0 >= 31u ? kFull : ((2u << w0) - 1u);
                 if (__ballot_sync(kFull, prior != 0u) & le0) {

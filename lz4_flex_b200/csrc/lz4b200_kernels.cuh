@@ -118,6 +118,20 @@ struct WordView {
         uint32_t a = __ldg(w + (x >> 2)), b = __ldg(w + (x >> 2) + 1);
         return __funnelshift_r(a, b, (x & 3u) * 8u);
     }
+    // ro4 in two steps: ro4_issue(ab, pos, on) loads the two words into ab for lanes with `on` (the other lanes issue no
+    // load and keep ab) and ro4_join(ab, pos) makes the 4 bytes of them.  The loads are opaque to the compiler, so two
+    // issues under complementary predicates stay two instructions with their own registers: a join of one waits for its
+    // lanes' data only.
+    __device__ __forceinline__ void ro4_issue(uint2 &ab, uint32_t pos, bool on) const
+    {
+        const uint32_t *q = w + ((pos + mis) >> 2);
+        asm volatile("{ .reg .pred p; setp.ne.u32 p, %3, 0; @p ld.global.nc.u32 %0, [%2]; @p ld.global.nc.u32 %1, [%2+4]; }"
+                     : "+r"(ab.x), "+r"(ab.y) : "l"(q), "r"((uint32_t)on));
+    }
+    __device__ __forceinline__ uint32_t ro4_join(uint2 ab, uint32_t pos) const
+    {
+        return __funnelshift_r(ab.x, ab.y, ((pos + mis) & 3u) * 8u);
+    }
     // 4 bytes at pos; requires only pos + 4 <= n (the second word is fetched only when it holds one of the 4 bytes)
     __device__ __forceinline__ uint32_t ro4s(uint32_t pos) const
     {
