@@ -492,6 +492,42 @@ lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx,
     uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
     lz4b200_frame_result *d_results, size_t nframes, void *stream);
 
+/* Device scratch lz4b200_frame_decompress_batch_device_async needs for nframes frames holding at most max_blocks
+ * blocks together (0 for nframes == 0; SIZE_MAX when either passes UINT32_MAX).  Host arithmetic only; no context, no
+ * device. */
+size_t lz4b200_frame_decompress_batch_device_async_scratch(size_t nframes, size_t max_blocks);
+
+/* lz4b200_frame_decompress_batch_device without host synchronisation, so the call can be captured in a CUDA graph and
+ * a host thread can enqueue the work that consumes the output right behind it.  Same arguments, plus a block capacity
+ * and a caller-owned scratch; every array, the scratch included, is device memory.
+ *   - Results: d_results[f] is what lz4b200_frame_decompress_next_device returns for region f with cap = d_out_cap[f],
+ *     on a context whose frame budget holds the frame in one group (equivalently, what
+ *     lz4b200_frame_decompress_batch_device gives on such a context: OUTPUT_FULL delivers nothing, the blocks before
+ *     a corrupt block are delivered), and d_out[d_out_off[f], +written) the bytes that call writes.  Nothing else of
+ *     d_out is written.  A region that holds several concatenated frames decodes only the first.
+ *   - Capacity: frame f is decoded only if the blocks its walk records for frames 0..f together number at most
+ *     max_blocks (a prefix rule: deterministic).  A frame past capacity gets status LZ4B200_INVALID_ARGUMENT in its
+ *     result with every other field 0, and nothing of its output is written; no decoded frame has that status, so the
+ *     caller can tell those frames apart and retry them with the synchronous call.
+ *   - No host synchronisation: the call makes no device-to-host copy, no copy from host memory, no allocation and no
+ *     synchronise, and keeps no state on the context's device memory (the decoders' ticket words are in the scratch,
+ *     reset on `stream`), so a captured call shares nothing with the context's other calls.  Everything is enqueued
+ *     on `stream` and the call returns at once; the results are ready when the stream reaches that point.
+ *   - INVALID_ARGUMENT, before anything is enqueued and with d_out and d_results untouched: a null ctx; a null array
+ *     or a null d_scratch with nframes > 0; nframes or max_blocks > UINT32_MAX; scratch_bytes below
+ *     lz4b200_frame_decompress_batch_device_async_scratch(nframes, max_blocks).  nframes == 0 does nothing.
+ *   - Every block is sized (its decoded length found without writing) before it is decoded, and then decodes straight
+ *     into d_out with exactly that length as its capacity, so no decoder writes past the region the sizing gave it.  A
+ *     frame whose decoder disagrees with the sizing on a block's status or length reports
+ *     LZ4B200_FRAME_DECOMPRESSION_ERROR with the decoder's block_status, never OK.
+ * The sizing pass costs device time the synchronous call does not spend (DESIGN.md §6); the per-block launches are
+ * sized by max_blocks, so a capacity far above the batch's block count costs some device time too. */
+lz4b200_status lz4b200_frame_decompress_batch_device_async(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+    uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+    lz4b200_frame_result *d_results, size_t nframes, size_t max_blocks,
+    void *d_scratch, size_t scratch_bytes, void *stream);
+
 /* ---- random access into one frame in DEVICE memory (no lz4_flex counterpart) ------------------------------------------
  * A frame records no decoded block sizes, so reading content bytes [a, b) of a frame means decoding it from its first
  * block.  lz4b200_frame_index_device builds, on the GPU, the decoded offset and length of every block without decoding

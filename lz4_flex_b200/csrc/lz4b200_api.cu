@@ -7,11 +7,13 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -566,12 +568,14 @@ __global__ void __launch_bounds__(128) frame_record_kernel(const uint8_t *in, co
     frames[g] = p;
 }
 
-// Block checksums, one thread per block of the group; frames[g].bad receives the first failing block of frame g.
+// Block checksums, one thread per block of the group; frames[g].bad receives the first failing block of frame g.  The
+// group holds nb blocks, or *nb_dev (at most nb) when the count is only known on the device.
 __global__ void __launch_bounds__(128) frame_batch_checksum_kernel(const uint8_t *in, const fw::FrameBlockDesc *desc,
-                                                                   const uint32_t *bframe, uint32_t nb, GroupFrame *frames)
+                                                                   const uint32_t *bframe, uint32_t nb, GroupFrame *frames,
+                                                                   const uint32_t *nb_dev = nullptr)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nb) return;
+    if (b >= nb || (nb_dev && b >= *nb_dev)) return;
     GroupFrame &p = frames[bframe[b]];
     if (!(p.walk->flg & 0x10)) return;
     if (!fw::block_checksum_ok(in + p.in_off, desc[b])) atomicMin(&p.bad, b - p.base);
@@ -693,6 +697,120 @@ __global__ void __launch_bounds__(128) frame_batch_digest_kernel(const GroupFram
     if (p.last && p.result->status == LZ4B200_OK && w.closed && w.has_checksum &&
         fw::xxh32_digest(*p.content) != w.content_checksum)
         p.result->status = LZ4B200_FRAME_CONTENT_CHECKSUM;
+}
+
+// ---- sync-free batch frame decoder (lz4b200_frame_decompress_batch_device_async) ---------------------------------------
+// The host knows the frame count and the block capacity `cap`, nothing else: every block count stays on the device, so
+// the per-block launches are sized by the capacity and their threads past the device count do nothing.  Every block is
+// sized before it is decoded, so it decodes straight into the caller's output with exactly its sized length as capacity.
+
+// The capacity rule, one CTA: the running sum of the blocks each frame's count walk recorded.  A frame whose blocks,
+// with those of the frames before it, pass `cap` is past capacity (over[f] = 1): its counts become 0, so the record walk
+// records none of its blocks.  *nb receives the blocks of the frames inside capacity.
+__global__ void __launch_bounds__(1024) frame_capacity_kernel(fw::FrameCount *counts, uint32_t *nb2, uint32_t n,
+                                                              uint64_t cap, uint8_t *over, uint32_t *nb)
+{
+    __shared__ uint64_t warp_sums[32];
+    __shared__ uint64_t carry;
+    __shared__ unsigned long long inside;
+    if (threadIdx.x == 0) { carry = 0; inside = 0; }
+    __syncthreads();
+    for (uint32_t base = 0; base < n; base += 1024) {
+        const uint32_t i = base + threadIdx.x;
+        const uint64_t v = i < n ? counts[i].nblocks : 0;
+        uint64_t x = v;
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(kFull, x, d);
+            if ((threadIdx.x & 31) >= d) x += y;
+        }
+        if ((threadIdx.x & 31) == 31) warp_sums[threadIdx.x >> 5] = x;
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            const uint64_t w = warp_sums[threadIdx.x];
+            uint64_t t = w;
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint64_t y = __shfl_up_sync(kFull, t, d);
+                if (threadIdx.x >= d) t += y;
+            }
+            warp_sums[threadIdx.x] = t - w;
+        }
+        __syncthreads();
+        const uint64_t incl = carry + warp_sums[threadIdx.x >> 5] + x;
+        if (i < n) {
+            const bool o = incl > cap;
+            over[i] = o;
+            if (o) { counts[i].nblocks = 0; nb2[i] = 0; nb2[n + i] = 0; }
+            else atomicMax(&inside, (unsigned long long)incl);
+        }
+        __syncthreads();
+        if (threadIdx.x == 1023) carry = incl;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *nb = (uint32_t)inside;
+}
+
+// The decoders' arguments, one thread per block up to the capacity: a block the result step delivers (glen > 0)
+// decodes at its gather offset with its sized length as capacity; the independent launch gets the compressed blocks of
+// independent frames, the linked launch those of linked frames (the blocks from *nind on), each in_len 0 for the
+// others.  The linked launch skips every block with stored_len != 0: its frame's stored blocks (history read from the
+// payload) and every block not of a linked frame.  Delivered stored blocks are copied from their payload (copy_len).
+__global__ void __launch_bounds__(128) frame_async_args_kernel(const GroupFrame *frames, const fw::FrameBlockDesc *desc,
+                                                               const uint32_t *bframe, const uint32_t *glen,
+                                                               const uint32_t *nb, const uint64_t *nind, uint32_t cap,
+                                                               uint64_t *in_off, uint32_t *in_len_ind,
+                                                               uint32_t *in_len_lnk, uint32_t *link_first,
+                                                               uint32_t *stored_len, uint32_t *done, uint32_t *copy_len)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= cap) return;
+    uint64_t off = 0;
+    uint32_t ind = 0, lnk = 0, first = 0, st = 1, copy = 0;
+    if (b < *nb) {
+        const GroupFrame &p = frames[bframe[b]];
+        const fw::FrameBlockDesc d = desc[b];
+        const bool stored = fw::block_stored(d), linked = b >= *nind;
+        off = p.in_off + d.payload_off;
+        if (stored) copy = glen[b];
+        else if (glen[b]) (linked ? lnk : ind) = fw::block_len(d);
+        if (linked) { first = p.base; st = stored ? fw::block_len(d) : 0u; }
+    }
+    in_off[b] = off;
+    in_len_ind[b] = ind;
+    in_len_lnk[b] = lnk;
+    link_first[b] = first;
+    stored_len[b] = st;
+    done[b] = 0;
+    copy_len[b] = copy;
+}
+
+// Every decoded block produced exactly its sized length: else mis[g] receives the first block of frame g that did not.
+__global__ void __launch_bounds__(128) frame_async_check_kernel(const fw::FrameBlockDesc *desc, const uint32_t *bframe,
+                                                                const uint32_t *glen, const uint32_t *out_len,
+                                                                const int32_t *status, const uint32_t *nb,
+                                                                uint32_t cap, uint32_t *mis)
+{
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= cap || b >= *nb || fw::block_stored(desc[b]) || !glen[b]) return;
+    if (status[b] != LZ4B200_OK || out_len[b] != glen[b]) atomicMin(mis + bframe[b], b);
+}
+
+// The results the sizing cannot decide, one thread per frame: a frame past capacity reports INVALID_ARGUMENT and
+// nothing else; a frame with a block the decoder disagreed on reports FRAME_DECOMPRESSION_ERROR with that block's
+// status, never OK.
+__global__ void __launch_bounds__(128) frame_async_finish_kernel(const uint8_t *over, const uint32_t *mis,
+                                                                 const int32_t *status, uint32_t n,
+                                                                 lz4b200_frame_result *results)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    if (over[f]) {
+        lz4b200_frame_result r{};
+        r.status = LZ4B200_INVALID_ARGUMENT;
+        results[f] = r;
+    } else if (mis[f] != fw::kNoBlock) {
+        results[f].status = LZ4B200_FRAME_DECOMPRESSION_ERROR;
+        results[f].block_status = status[mis[f]];
+    }
 }
 
 }  // namespace lz4b200
@@ -2843,9 +2961,26 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
     return (lz4b200_status)r.status;
 }
 
-// The record walk and block checksums of the batch's frames [f0, f0 + gn), whose nb blocks were counted by
-// frame_count_kernel into ctx->d_fwalk, d_fcount and d_fnb: descriptors at ctx->d_desc, each block's frame at
-// ctx->d_bframe, one GroupFrame per frame at ctx->d_gframe, all enqueued on s.
+// The record walk and block checksums of the batch's frames [f0, f0 + gn), whose blocks frame_count_kernel counted into
+// walks, counts and nb2: the scans of the two block-count classes at scan (2 x (gn + 1)), descriptors at desc, each
+// block's frame at bframe, one GroupFrame per frame at frames, all enqueued on s.  The frames hold nb blocks, or *nb_dev
+// (at most nb) when the count is only known on the device.
+void enqueue_record(cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+                    const uint64_t *d_out_off, const uint64_t *d_out_cap, const fw::FrameWalk *walks,
+                    const fw::FrameCount *counts, const uint32_t *nb2, uint64_t *scan, lz4b200_xxh32_state *states,
+                    lz4b200_frame_result *d_results, uint32_t nframes, uint32_t f0, uint32_t gn, uint32_t nb,
+                    const uint32_t *nb_dev, fw::FrameBlockDesc *desc, uint32_t *bframe, GroupFrame *frames)
+{
+    uint64_t *scan_ind = scan, *scan_lnk = scan + gn + 1;
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(nb2 + f0, scan_ind, gn);
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(nb2 + nframes + f0, scan_lnk, gn);
+    frame_record_kernel<<<(gn + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, f0, gn,
+                                                         walks, counts, scan_ind, scan_lnk, desc, bframe, states,
+                                                         d_results, frames);
+    if (nb) frame_batch_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, desc, bframe, nb, frames, nb_dev);
+}
+
+// The same over ctx->d_fwalk, d_fcount and d_fnb, into ctx->d_fscan, d_desc, d_bframe and d_gframe.
 lz4b200_status record_frames(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off,
                              const uint64_t *d_frame_len, const uint64_t *d_out_off, const uint64_t *d_out_cap,
                              lz4b200_xxh32_state *states, lz4b200_frame_result *d_results, uint32_t nframes,
@@ -2853,16 +2988,9 @@ lz4b200_status record_frames(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_
 {
     CTX_CUDA(ctx, ctx->d_fscan.reserve(2 * (size_t)(gn + 1))); CTX_CUDA(ctx, ctx->d_gframe.reserve(gn));
     CTX_CUDA(ctx, ctx->d_desc.reserve(nb)); CTX_CUDA(ctx, ctx->d_bframe.reserve(nb));
-    uint64_t *scan_ind = ctx->d_fscan.p, *scan_lnk = ctx->d_fscan.p + gn + 1;
-
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + f0, scan_ind, gn);
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_fnb.p + nframes + f0, scan_lnk, gn);
-    frame_record_kernel<<<(gn + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, f0, gn,
-                                                         ctx->d_fwalk.p, ctx->d_fcount.p, scan_ind, scan_lnk,
-                                                         ctx->d_desc.p, ctx->d_bframe.p, states, d_results,
-                                                         ctx->d_gframe.p);
-    if (nb) frame_batch_checksum_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, nb,
-                                                                        ctx->d_gframe.p);
+    enqueue_record(s, d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, ctx->d_fwalk.p, ctx->d_fcount.p,
+                   ctx->d_fnb.p, ctx->d_fscan.p, states, d_results, nframes, f0, gn, nb, nullptr, ctx->d_desc.p,
+                   ctx->d_bframe.p, ctx->d_gframe.p);
     CTX_CUDA(ctx, cudaGetLastError());
     return LZ4B200_OK;
 }
@@ -3043,6 +3171,22 @@ lz4b200_status lz4b200_frame_decompress(lz4b200_ctx *ctx, const uint8_t *in, siz
 // ---- frame index and range decode (no lz4_flex counterpart) ------------------------------------------------------------
 namespace {
 
+// The frame decoders' result step from sized blocks, shared by the index and the sync-free batch decoder: one sizing
+// thread per block of the gn frames at `frames` (nb blocks, or *nb_dev of them, at most nb, when the count is only known
+// on the device), the linked frames' reach check, then frame_resolve_kernel, which gives each frame's result except
+// the content checksum and each block's gather offset and length.  Everything is enqueued on s.
+void enqueue_sized_resolve(cudaStream_t s, const uint8_t *d_in, GroupFrame *frames, uint32_t gn, uint32_t nb,
+                           const uint32_t *nb_dev, const fw::FrameBlockDesc *desc, const uint32_t *bframe,
+                           uint32_t *len, int32_t *status, uint64_t *expected, uint32_t *cap, uint32_t *reach,
+                           uint64_t *gdst, uint32_t *glen, uint8_t *hash)
+{
+    const uint32_t fgrid = (gn + 3) / 4;
+    if (nb) fr::block_size_kernel<<<(nb + 127) / 128, 128, 0, s>>>(d_in, desc, bframe, frames, nb, len, status, expected,
+                                                                   cap, reach, nb_dev);
+    fr::frame_reach_kernel<<<fgrid, 128, 0, s>>>(frames, gn, reach, status, expected, len);
+    frame_resolve_kernel<<<fgrid, 128, 0, s>>>(frames, gn, desc, len, status, expected, cap, gdst, glen, hash);
+}
+
 // The index after the walk, shared by the one-frame and the batch call: the gn frames at ctx->d_gframe, whose nb blocks
 // are described at ctx->d_desc and ctx->d_bframe (each frame's bad: its first block that fails its checksum).  One
 // sizing thread per block, the linked frames' reach check, then the frame decoders' own result step (each frame one
@@ -3052,20 +3196,15 @@ namespace {
 lz4b200_status index_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, uint32_t gn, uint32_t nb,
                            const uint64_t *entry_off, lz4b200_frame_index_entry *index, lz4b200_frame_index_info *info)
 {
-    const uint32_t grid = (nb + 127) / 128, fgrid = (gn + 3) / 4;
+    const uint32_t grid = (nb + 127) / 128;
     CTX_CUDA(ctx, ctx->d_fhash.reserve(gn)); CTX_CUDA(ctx, ctx->d_out_len.reserve(nb));
     CTX_CUDA(ctx, ctx->d_status.reserve(nb)); CTX_CUDA(ctx, ctx->d_expected.reserve(nb));
     CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb)); CTX_CUDA(ctx, ctx->d_reach.reserve(nb));
     CTX_CUDA(ctx, ctx->d_gdst.reserve(nb)); CTX_CUDA(ctx, ctx->d_glen.reserve(nb));
     GroupFrame *frames = ctx->d_gframe.p;
-    if (nb) fr::block_size_kernel<<<grid, 128, 0, s>>>(d_in, ctx->d_desc.p, ctx->d_bframe.p, frames, nb, ctx->d_out_len.p,
-                                                       ctx->d_status.p, ctx->d_expected.p, ctx->d_out_cap.p,
-                                                       ctx->d_reach.p);
-    fr::frame_reach_kernel<<<fgrid, 128, 0, s>>>(frames, gn, ctx->d_reach.p, ctx->d_status.p, ctx->d_expected.p,
-                                                 ctx->d_out_len.p);
-    frame_resolve_kernel<<<fgrid, 128, 0, s>>>(frames, gn, ctx->d_desc.p, ctx->d_out_len.p, ctx->d_status.p,
-                                               ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_gdst.p, ctx->d_glen.p,
-                                               ctx->d_fhash.p);
+    enqueue_sized_resolve(s, d_in, frames, gn, nb, nullptr, ctx->d_desc.p, ctx->d_bframe.p, ctx->d_out_len.p,
+                          ctx->d_status.p, ctx->d_expected.p, ctx->d_out_cap.p, ctx->d_reach.p, ctx->d_gdst.p,
+                          ctx->d_glen.p, ctx->d_fhash.p);
     if (nb) fr::index_entries_kernel<<<grid, 128, 0, s>>>(ctx->d_desc.p, ctx->d_bframe.p, frames, ctx->d_gdst.p,
                                                           ctx->d_glen.p, nb, entry_off, index);
     fr::index_info_kernel<<<(gn + 127) / 128, 128, 0, s>>>(frames, gn, info);
@@ -3204,6 +3343,107 @@ lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t 
         }
     }
     CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    return LZ4B200_OK;
+}
+
+// ---- sync-free batch frame decoder ---------------------------------------------------------------------------------------
+namespace {
+
+// The caller's scratch of lz4b200_frame_decompress_batch_device_async, carved into 256-byte aligned arrays: per frame
+// (n) the count walk, the scans, the GroupFrame, the content hash and the capacity and check flags; per block (cap) the
+// record walk, the sizing, and the decoders' arguments and results; the decoders' ticket words and the block count.
+// With a null base only `bytes` is meaningful.
+struct AsyncScratch {
+    fw::FrameWalk *walks;
+    fw::FrameCount *counts;
+    uint32_t *nb2, *mis;
+    uint64_t *scan;
+    GroupFrame *frames;
+    lz4b200_xxh32_state *content;
+    uint8_t *hash, *over;
+    fw::FrameBlockDesc *desc;
+    uint32_t *bframe, *len, *cap, *reach, *glen, *in_len_ind, *in_len_lnk, *link_first, *stored_len, *done, *copy_len;
+    int32_t *status;
+    uint64_t *expected, *gdst, *in_off;
+    uint32_t *tickets, *nb;
+    size_t bytes = 0;
+
+    AsyncScratch(void *base, size_t n, size_t nblocks)
+    {
+        auto take = [&](auto *&p, size_t count) {
+            p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + bytes);
+            bytes += (count * sizeof(*p) + 255) & ~size_t(255);
+        };
+        take(walks, n); take(counts, n); take(nb2, 2 * n); take(mis, n); take(scan, 2 * (n + 1)); take(frames, n);
+        take(content, n); take(hash, n); take(over, n);
+        take(desc, nblocks); take(bframe, nblocks); take(len, nblocks); take(cap, nblocks); take(reach, nblocks);
+        take(glen, nblocks); take(in_len_ind, nblocks); take(in_len_lnk, nblocks); take(link_first, nblocks);
+        take(stored_len, nblocks); take(done, nblocks); take(copy_len, nblocks); take(status, nblocks);
+        take(expected, nblocks); take(gdst, nblocks); take(in_off, nblocks);
+        take(tickets, 4); take(nb, 1);
+    }
+};
+
+}  // namespace
+
+size_t lz4b200_frame_decompress_batch_device_async_scratch(size_t nframes, size_t max_blocks)
+{
+    if (nframes > 0xffffffffull || max_blocks > 0xffffffffull) return SIZE_MAX;
+    return nframes ? AsyncScratch(nullptr, nframes, max_blocks).bytes : 0;
+}
+
+// Many frames with no host synchronisation: count walk, capacity rule, record walk and block checksums, sizing and the
+// result step, then the decoders write each delivered block in place, a check that they agree with the sizing, and the
+// content checksums.  Nothing is read back, allocated or reserved; every launch is sized by nframes or max_blocks.
+lz4b200_status lz4b200_frame_decompress_batch_device_async(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                           const uint64_t *d_frame_off, const uint64_t *d_frame_len,
+                                                           uint8_t *d_out, const uint64_t *d_out_off,
+                                                           const uint64_t *d_out_cap, lz4b200_frame_result *d_results,
+                                                           size_t nframes, size_t max_blocks, void *d_scratch,
+                                                           size_t scratch_bytes, void *stream)
+{
+    if (!ctx || nframes > 0xffffffffull || max_blocks > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_frame_off || !d_frame_len || !d_out || !d_out_off || !d_out_cap || !d_results ||
+                    !d_scratch))
+        return LZ4B200_INVALID_ARGUMENT;
+    if (scratch_bytes < lz4b200_frame_decompress_batch_device_async_scratch(nframes, max_blocks))
+        return LZ4B200_INVALID_ARGUMENT;
+    if (!nframes) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t n = (uint32_t)nframes, cap = (uint32_t)max_blocks, fgrid = (n + 127) / 128, bgrid = (cap + 127) / 128;
+    AsyncScratch m(d_scratch, n, cap);
+    CTX_CUDA(ctx, cudaMemsetAsync(m.tickets, 0, 4 * sizeof(uint32_t), s));
+    CTX_CUDA(ctx, cudaMemsetAsync(m.mis, 0xff, n * sizeof(uint32_t), s));
+    frame_count_kernel<<<fgrid, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ~0ull, m.walks, m.counts, m.nb2);
+    frame_capacity_kernel<<<1, 1024, 0, s>>>(m.counts, m.nb2, n, cap, m.over, m.nb);
+    enqueue_record(s, d_in, d_frame_off, d_frame_len, d_out_off, d_out_cap, m.walks, m.counts, m.nb2, m.scan, m.content,
+                   d_results, n, 0, n, cap, m.nb, m.desc, m.bframe, m.frames);
+    enqueue_sized_resolve(s, d_in, m.frames, n, cap, m.nb, m.desc, m.bframe, m.len, m.status, m.expected, m.cap,
+                          m.reach, m.gdst, m.glen, m.hash);
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (cap) {
+        frame_async_args_kernel<<<bgrid, 128, 0, s>>>(m.frames, m.desc, m.bframe, m.glen, m.nb, m.scan + n, cap, m.in_off,
+                                                      m.in_len_ind, m.in_len_lnk, m.link_first, m.stored_len, m.done,
+                                                      m.copy_len);
+        CTX_CUDA(ctx, cudaGetLastError());
+        // both launches over the whole capacity: which blocks are linked is known only on the device
+        BatchArgs a{d_in, m.in_off, m.in_len_ind, nullptr, d_out, m.gdst, m.glen, m.len, m.status, nullptr, cap, nullptr};
+        const lz4b200_status st = launch_decompress(ctx, a, s, m.tickets);
+        if (st != LZ4B200_OK) return st;
+        BatchArgs l{d_in, m.in_off, m.in_len_lnk, nullptr, d_out, m.gdst, m.glen, m.len, m.status, nullptr, cap,
+                    m.tickets + 2};
+        l.link_first = m.link_first; l.stored_off = m.in_off; l.stored_len = m.stored_len; l.done = m.done;
+        lz4_decompress_blocks_linked<32><<<std::min<uint32_t>((cap + 3) / 4, (uint32_t)ctx->sm_count * 8), 128, 0, s>>>(l);
+        GatherArgs g{d_in, nullptr, m.in_off, nullptr, m.copy_len, nullptr, nullptr, nullptr, d_out, m.gdst, cap};
+        gather_segments_kernel<<<std::min<uint32_t>(cap, (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
+        frame_async_check_kernel<<<bgrid, 128, 0, s>>>(m.desc, m.bframe, m.glen, m.len, m.status, m.nb, cap, m.mis);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    frame_batch_hash_kernel<<<n, 256, 0, s>>>(d_out, m.frames, m.hash);
+    frame_batch_digest_kernel<<<fgrid, 128, 0, s>>>(m.frames, n, m.hash);
+    frame_async_finish_kernel<<<fgrid, 128, 0, s>>>(m.over, m.mis, m.status, n, d_results);
+    CTX_CUDA(ctx, cudaGetLastError());
     return LZ4B200_OK;
 }
 

@@ -78,14 +78,15 @@ __device__ __forceinline__ SizeResult size_block(const uint8_t *__restrict__ src
 // One thread per block of an index group (the GroupFrames of the frame decoders' result step, one per frame): its
 // decoded length, status, OutputTooSmall expected and capacity (the frame decoders' out_cap, min(block size, 255 x
 // payload)), and a linked block's reach.  The block's frame gives the payload's place, the block size and the block
-// mode.  A stored block is its payload.
+// mode.  A stored block is its payload.  The group holds nb blocks, or *nb_dev (at most nb) when the count is only known
+// on the device.
 __global__ void __launch_bounds__(128) block_size_kernel(const uint8_t *in, const fw::FrameBlockDesc *desc,
                                                          const uint32_t *bframe, const GroupFrame *frames, uint32_t nb,
                                                          uint32_t *len, int32_t *status, uint64_t *expected,
-                                                         uint32_t *cap, uint32_t *reach)
+                                                         uint32_t *cap, uint32_t *reach, const uint32_t *nb_dev = nullptr)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nb) return;
+    if (b >= nb || (nb_dev && b >= *nb_dev)) return;
     const GroupFrame &p = frames[bframe[b]];
     const uint64_t bs = p.walk->bs;
     const fw::FrameBlockDesc d = desc[b];

@@ -424,6 +424,62 @@ def decompress_frames_device(d_in, offsets, lengths, out=None, out_offsets=None,
     return DecodedFrames(out, oo, results)
 
 
+def default_max_blocks(in_len: int, nframes: int) -> int:
+    """The block capacity decompress_frames_device_async() assumes when none is given: in_len // 256 + nframes.  Every
+    block of a frame but its last holds at least 64 KiB, and LZ4 cannot store 64 KiB in much less than 256 bytes (the
+    densest block of 64 KiB, all one byte, takes 257 bytes of payload plus its 4-byte BlockInfo), so a frame of k bytes
+    written with full blocks has at most k // 256 + 1 blocks."""
+    return in_len // 256 + nframes
+
+
+def decompress_frames_device_async(d_in, offsets, lengths, out, out_offsets, out_caps, max_blocks: int | None = None,
+                                   ctx: _block.Context | None = None, stream: int | None = None) -> DecodedFrames:
+    """decompress_frames_device() without synchronising the host (lz4b200_frame_decompress_batch_device_async): the
+    work is enqueued on torch's current stream (or `stream`) and the call returns at once, so it can be captured in a
+    CUDA graph (torch.cuda.graph).  Frame i's result is what decompress_frames_device() gives for it on a context whose
+    frame budget holds the frame in one group; the returned DecodedFrames holds the device results tensor, valid once
+    the stream has reached the call.
+
+    out, out_offsets and out_caps are required: sizing the output would need a readback.  Offsets, lengths and caps
+    may be int64 sequences, but under graph capture they must already be int64 CUDA tensors (a copy from host memory
+    cannot be captured); a replay reads them, and d_in, where they are then.
+
+    max_blocks bounds the blocks the frames hold together (default: default_max_blocks(d_in.numel(), nframes), which
+    holds for frames written with full blocks, as every encoder here writes them).  Frames flushed with short blocks
+    can hold more.  Frame i is decoded only if frames 0..i hold at most max_blocks blocks together; a frame past that
+    gets ValueError as its error (status LZ4B200_INVALID_ARGUMENT, every other result field 0) and none of its
+    output is written; decompress_frames_device() decodes it.  The scratch (lz4b200_frame_decompress_batch_device_async_scratch bytes, about 100
+    bytes per block of capacity) is allocated with torch.empty, so under capture it comes from the graph's pool."""
+    import torch
+    _device_u8(d_in, "d_in")
+    _device_u8(out, "out")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    L = _native.lib()
+    with torch.cuda.stream(torch.cuda.ExternalStream(s, device=dev)):
+        # everything on the call's stream: copies of host sequences are ordered before the decode, and the caching
+        # allocator reuses these tensors' memory only after the work that reads them
+        offs, lens = _device_i64(offsets, dev, "offsets"), _device_i64(lengths, dev, "lengths")
+        oo, caps = _device_i64(out_offsets, dev, "out_offsets"), _device_i64(out_caps, dev, "out_caps")
+        n = offs.numel()
+        if lens.numel() != n or oo.numel() != n or caps.numel() != n:
+            raise ValueError("offsets, lengths, out_offsets and out_caps need one entry per frame")
+        if max_blocks is None:
+            max_blocks = default_max_blocks(d_in.numel(), n)
+        if max_blocks < 0:
+            raise ValueError("max_blocks must not be negative")
+        nbytes = L.lz4b200_frame_decompress_batch_device_async_scratch(n, max_blocks)
+        results = torch.empty((n, 5), dtype=torch.int64, device=dev)
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    st = L.lz4b200_frame_decompress_batch_device_async(
+        ctx.handle, d_in.data_ptr() if d_in.numel() else None, offs.data_ptr(), lens.data_ptr(), out.data_ptr(),
+        oo.data_ptr(), caps.data_ptr(), results.data_ptr(), n, max_blocks, scratch.data_ptr(), nbytes, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return DecodedFrames(out, oo, results)
+
+
 _CONTENT_CHECKSUM = 108
 
 
