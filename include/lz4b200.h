@@ -382,6 +382,63 @@ lz4b200_status lz4b200_frame_compress_linked_batch_device(lz4b200_ctx *ctx,
     uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
     size_t nframes, void *stream);
 
+/* Device scratch lz4b200_frame_compress_batch_device_async (and its linked form) needs on ctx for nframes frames holding
+ * at most max_blocks blocks and max_in_bytes input bytes together: 0 for nframes == 0; SIZE_MAX for a null ctx, when
+ * nframes or max_blocks passes UINT32_MAX, or when max_in_bytes passes any device's memory.  About 1.1 bytes per input
+ * byte (the encoders' slots) and 60 per block of capacity.  It takes the context because the context's encoder shape
+ * decides whether the scratch holds a global hash-table region: the default shape keeps every table in shared memory
+ * and needs none.  Host arithmetic only. */
+size_t lz4b200_frame_compress_batch_device_async_scratch(const lz4b200_ctx *ctx, size_t nframes, size_t max_blocks,
+                                                         size_t max_in_bytes);
+
+/* lz4b200_frame_compress_batch_device without host synchronisation, so the call can be captured in a CUDA graph and a
+ * host thread can enqueue the work that consumes the frames right behind it.  Input f is d_in[d_in_off[f],
+ * d_in_off[f] + d_in_len[f]); every array, the scratch included, is DEVICE memory, and only *info is read on the host.
+ *   - Same bytes: for every frame inside the capacity, d_out[d_frame_off[f], d_frame_off[f + 1]) is exactly what
+ *     lz4b200_frame_compress_batch_device writes for the same inputs and info (Auto resolves per frame from its length;
+ *     with has_content_size the header records that frame's length), and d_status[f] == LZ4B200_OK.  Frames lie back to
+ *     back from d_out[0]; d_frame_off[nframes] is the end, and nothing of d_out past it is written.
+ *   - Capacity, a prefix rule (deterministic): frame f is compressed only if frames 0..f together hold at most
+ *     max_blocks blocks and max_in_bytes input bytes, and the sum of their lz4b200_frame_bound(d_in_len[g], &info_g) is
+ *     at most out_cap.  A frame past capacity (the first, and every frame after it) writes nothing, and
+ *     d_frame_off[f] == d_frame_off[f + 1] == the end of the last frame compressed.  Its d_status[f] is the first limit
+ *     frames 0..f pass, checked in the order blocks, input bytes, bound: LZ4B200_INVALID_ARGUMENT for the first two,
+ *     LZ4B200_COMPRESS_OUTPUT_TOO_SMALL for out_cap.  The caller can hand those frames to the synchronous call.
+ *   - No host synchronisation: the call makes no device-to-host copy, no copy from host memory, no allocation and no
+ *     synchronise, and keeps no state on the context's device memory: the plans, the encoders' slots, their ticket words
+ *     (reset on `stream`) and any global-table region are in d_scratch, so a captured call shares nothing with the
+ *     context's other calls.  *info reaches the device as a kernel argument.  Everything is enqueued on `stream` and the
+ *     call returns at once; the results are ready when the stream reaches that point.
+ *   - INVALID_ARGUMENT, before anything is enqueued and with d_out, d_frame_off and d_status untouched, in this order: a
+ *     null ctx, info or d_frame_off; a null d_in, d_in_off, d_in_len, d_status or d_scratch with nframes > 0, or a null
+ *     d_out with out_cap > 0 (with out_cap == 0 no frame fits and nothing is written);
+ *     nframes or max_blocks above UINT32_MAX; a block size id other than 0 or 4..7; then FRAME_LINKED_UNSUPPORTED for
+ *     info->linked (INVALID_ARGUMENT for !info->linked in the linked form), as the synchronous calls answer it; then
+ *     INVALID_ARGUMENT for scratch_bytes below lz4b200_frame_compress_batch_device_async_scratch(ctx, nframes,
+ *     max_blocks, max_in_bytes).  Input ranges are not checked against d_in.  nframes == 0 sets d_frame_off[0] = 0 on
+ *     the stream.
+ * The frames are planned on the device by one CTA, and the per-block launches are sized by max_blocks, so a capacity
+ * far above the batch's block count costs some device time.  The block lengths are not known on the host: with a block
+ * size other than 64 KiB, or Auto, both encoder table widths run (DESIGN.md §6).  d_in and d_out may have any
+ * alignment and must not overlap. */
+lz4b200_status lz4b200_frame_compress_batch_device_async(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_in_off, const uint64_t *d_in_len,
+    const lz4b200_frame_info *info,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off, int32_t *d_status,
+    size_t nframes, size_t max_blocks, size_t max_in_bytes,
+    void *d_scratch, size_t scratch_bytes, void *stream);
+
+/* The same for BlockMode::Linked, the sync-free form of lz4b200_frame_compress_linked_batch_device: same bytes for every
+ * frame inside capacity, same capacity rule, scratch and argument errors.  The chains start in frame index order, not
+ * longest first as in the synchronous call: the bytes do not depend on the order, only the time does (a batch whose
+ * longest frames come last takes longer). */
+lz4b200_status lz4b200_frame_compress_linked_batch_device_async(lz4b200_ctx *ctx,
+    const uint8_t *d_in, const uint64_t *d_in_off, const uint64_t *d_in_len,
+    const lz4b200_frame_info *info,
+    uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off, int32_t *d_status,
+    size_t nframes, size_t max_blocks, size_t max_in_bytes,
+    void *d_scratch, size_t scratch_bytes, void *stream);
+
 /* Block-range form used for multi-GPU sharding (SURVEY.md §8e): compress frame blocks
  * [first_block, first_block + nblocks) of a stream cut into `block_size`-byte blocks.  `d_in`
  * points at the first byte of block `first_block` (device memory, `in_len` bytes for this

@@ -155,6 +155,11 @@ SIGNATURES = {
     "lz4b200_frame_compress_batch_device": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp, _sz, _vp]),
     "lz4b200_frame_compress_linked_batch_device": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp, _sz,
                                                            _vp]),
+    "lz4b200_frame_compress_batch_device_async_scratch": (_sz, [_vp, _sz, _sz, _sz]),
+    "lz4b200_frame_compress_batch_device_async": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp, _vp,
+                                                         _sz, _sz, _sz, _vp, _sz, _vp]),
+    "lz4b200_frame_compress_linked_batch_device_async": (_i32, [_vp, _vp, _vp, _vp, C.POINTER(FrameInfoC), _vp, _sz, _vp,
+                                                                _vp, _sz, _sz, _sz, _vp, _sz, _vp]),
     "lz4b200_frame_compress_blocks_device": (_i32, [_vp, _vp, _sz, _sz, C.c_uint64, _vp, _sz, _vp, _vp, _vp]),
     "lz4b200_frame_blocks_bound": (_sz, [_sz, _sz]),
     "lz4b200_frame_range_compress": (_i32, [_vp, _vp, _sz, _sz, C.c_uint64, _vp, _vp, _vp]),

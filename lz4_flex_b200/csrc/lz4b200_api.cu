@@ -39,7 +39,7 @@ namespace lz4b200 {
 
 // Exclusive scan of sizes[0..n) into offs[0..n], offs[n] = total.  One CTA; n is a block count
 // (<= a few 100k), so a single-CTA chunked scan is far below launch noise.
-__global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint32_t *sizes, uint64_t *offs, uint32_t n)
+__device__ __forceinline__ void scan_sizes(const uint32_t *sizes, uint64_t *offs, uint32_t n)
 {
     __shared__ uint64_t warp_sums[32];
     __shared__ uint64_t carry;
@@ -72,6 +72,19 @@ __global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint32_t *sizes,
     if (threadIdx.x == 0) offs[n] = carry;
 }
 
+// The kernels the frame encoders' pipeline shares with the sync-free batch call (enqueue_frames) cover a block count
+// known only on the device, *n_dev (at most n), when given one.  The scan, the gather and the block info take it in an
+// overload of their own, so that the form the synchronous calls run keeps its code and registers.
+__global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint32_t *sizes, uint64_t *offs, uint32_t n)
+{
+    scan_sizes(sizes, offs, n);
+}
+__global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint32_t *sizes, uint64_t *offs, uint32_t n,
+                                                          const uint32_t *n_dev)
+{
+    scan_sizes(sizes, offs, min(n, *n_dev));
+}
+
 // Generic gather: segment b copies len[b] bytes from src_base[sel] + src_off[b] to dst + dst_off[b],
 // optionally preceded by a 4-byte little-endian word (the frame BlockInfo).  One CTA per segment
 // slice; byte-granular head/tail, 16-byte body when co-aligned.
@@ -90,9 +103,9 @@ struct GatherArgs {
     const uint64_t *dst_shift = nullptr;   // optional device scalar added to every destination offset
 };
 
-__global__ void __launch_bounds__(256) gather_segments_kernel(GatherArgs g)
+__device__ __forceinline__ void gather_segments(const GatherArgs &g, uint32_t nseg)
 {
-    for (uint32_t b = blockIdx.x; b < g.nseg; b += gridDim.x) {
+    for (uint32_t b = blockIdx.x; b < nseg; b += gridDim.x) {
         const bool second = g.pick && g.pick[b];
         const uint8_t *s = second ? g.src_b + g.off_b[b] : g.src_a + g.off_a[b];
         const uint32_t len = second ? g.len_b[b] : g.len_a[b];
@@ -118,21 +131,46 @@ __global__ void __launch_bounds__(256) gather_segments_kernel(GatherArgs g)
     }
 }
 
+__global__ void __launch_bounds__(256) gather_segments_kernel(GatherArgs g) { gather_segments(g, g.nseg); }
+
+// The segments [0, *nseg_dev) of at most g.nseg.
+__global__ void __launch_bounds__(256) gather_segments_kernel(GatherArgs g, const uint32_t *nseg_dev)
+{
+    gather_segments(g, min(g.nseg, *nseg_dev));
+}
+
 // Frame encoder bookkeeping for a block range: per block, decide compressed-vs-stored
 // (frame/compress.rs:301-306) and produce BlockInfo word + segment size.  `trailer` (0, or 4 for a
 // block checksum) is reserved after each payload.
-__global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t n, uint32_t trailer,
-                                        uint32_t *info_word, uint8_t *pick_raw, uint32_t *seg_size,
-                                        uint32_t *payload_len)
+__device__ __forceinline__ void frame_block_info(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t i,
+                                                 uint32_t trailer, uint32_t *info_word, uint8_t *pick_raw,
+                                                 uint32_t *seg_size, uint32_t *payload_len)
 {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
     uint32_t c = comp_len[i], r = raw_len[i];
     bool stored = !(c < r);
     info_word[i] = stored ? (r | 0x80000000u) : c;
     pick_raw[i] = stored ? 1 : 0;
     payload_len[i] = stored ? r : c;
     seg_size[i] = 4u + (stored ? r : c) + trailer;
+}
+
+__global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t n, uint32_t trailer,
+                                        uint32_t *info_word, uint8_t *pick_raw, uint32_t *seg_size,
+                                        uint32_t *payload_len)
+{
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    frame_block_info(comp_len, raw_len, i, trailer, info_word, pick_raw, seg_size, payload_len);
+}
+
+// The blocks [0, *n_dev) of at most n.
+__global__ void frame_block_info_kernel(const uint32_t *comp_len, const uint32_t *raw_len, uint32_t n, uint32_t trailer,
+                                        uint32_t *info_word, uint8_t *pick_raw, uint32_t *seg_size,
+                                        uint32_t *payload_len, const uint32_t *n_dev)
+{
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || i >= *n_dev) return;
+    frame_block_info(comp_len, raw_len, i, trailer, info_word, pick_raw, seg_size, payload_len);
 }
 
 // Descriptor generator for a run of equal-sized blocks cut from one contiguous buffer.
@@ -375,12 +413,14 @@ __global__ void __launch_bounds__(256) content_hash_kernel(lz4b200_xxh32_state *
 __global__ void xxh32_reset_kernel(lz4b200_xxh32_state *st, uint32_t seed) { fw::xxh32_reset(*st, seed); }
 
 // Block checksums of a packed range (frame/compress.rs:313-316): the XXH32 of each payload as written (compressed or
-// stored), stored little-endian in the 4 trailer bytes after it.  One thread per block.
+// stored), stored little-endian in the 4 trailer bytes after it.  One thread per block of the first n, or of the first
+// *n_dev (at most n).
 __global__ void __launch_bounds__(128) frame_block_checksum_kernel(uint8_t *dst, const uint64_t *seg_off,
-                                                                   const uint32_t *payload_len, uint32_t n)
+                                                                   const uint32_t *payload_len, uint32_t n,
+                                                                   const uint32_t *n_dev = nullptr)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= n || (n_dev && i >= *n_dev)) return;
     uint8_t *payload = dst + seg_off[i] + 4;
     const uint32_t len = payload_len[i];
     const uint32_t h = fw::xxh32(payload, len, 0);
@@ -432,13 +472,20 @@ static_assert(sizeof(fb::FramePlan) == 64, "one frame's plan is 64 bytes");
 __global__ void frame_plan_store_kernel(fb::FramePlan *dst, fb::FramePlan p) { *dst = p; }
 
 // The compressor's arguments, one thread per block of the batch (fb::batch_block); dst[b] receives the block's shift
-// into the packed output, to which frame_batch_dst_kernel adds the scan of the segment sizes.
+// into the packed output, to which frame_batch_dst_kernel adds the scan of the segment sizes.  With nb_dev the batch
+// holds *nb_dev (at most nb) blocks: each of the nb threads past it gives an empty input with no room, which every
+// encoder reports as COMPRESS_OUTPUT_TOO_SMALL without reading or writing any byte.
 __global__ void __launch_bounds__(128) frame_batch_blocks_kernel(const fb::FramePlan *plan, uint32_t nframes, uint32_t nb,
                                                                  uint64_t *in_off, uint32_t *in_len, uint64_t *out_off,
-                                                                 uint32_t *out_cap, uint8_t *flags, uint64_t *dst)
+                                                                 uint32_t *out_cap, uint8_t *flags, uint64_t *dst,
+                                                                 const uint32_t *nb_dev = nullptr)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
+    if (nb_dev && b >= *nb_dev) {
+        in_off[b] = 0; in_len[b] = 0; out_off[b] = 0; out_cap[b] = 0; flags[b] = LZ4B200_BLOCK_HASH5_ALWAYS; dst[b] = 0;
+        return;
+    }
     const fb::BlockJob j = fb::batch_block(plan, nframes, b);
     in_off[b] = j.in_off;
     in_len[b] = j.in_len;
@@ -449,11 +496,14 @@ __global__ void __launch_bounds__(128) frame_batch_blocks_kernel(const fb::Frame
 }
 
 // With pos_in, the blocks land *pos_in bytes further (a streaming group at its call's position) and thread 0 stores
-// their end to *pos_out, another word than the *pos_in every thread reads.
+// their end to *pos_out, another word than the *pos_in every thread reads.  With nb_dev the batch holds *nb_dev (at
+// most nb) blocks.
 __global__ void __launch_bounds__(128) frame_batch_dst_kernel(const uint64_t *seg_off, uint32_t nb, uint64_t *dst,
-                                                              const uint64_t *pos_in, uint64_t *pos_out)
+                                                              const uint64_t *pos_in, uint64_t *pos_out,
+                                                              const uint32_t *nb_dev = nullptr)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (nb_dev) nb = min(nb, *nb_dev);
     const uint64_t pos = pos_in ? *pos_in : 0;
     if (b < nb) dst[b] += seg_off[b] + pos;
     if (b == 0 && pos_out) *pos_out = pos + seg_off[nb];
@@ -472,7 +522,9 @@ __global__ void __launch_bounds__(256, 1) frame_batch_content_kernel(const uint8
 }
 
 // Everything of each frame but its blocks, one thread per frame (frame/compress.rs:209-230): the header, the EndMark,
-// the content digest when `states` is given, and frame_off[f]; the last frame's thread also writes the total.
+// the content digest when `states` is given, and frame_off[f]; the last frame's thread also writes the total.  A frame
+// without a header (past the capacity of the sync-free call, fb::drop_frame) writes only frame_off[f]: it has no
+// blocks, so it starts and ends where the frame before it ends.
 __global__ void __launch_bounds__(128) frame_batch_tail_kernel(uint8_t *out, const fb::FramePlan *plan, uint32_t n,
                                                                const uint64_t *seg_off, const lz4b200_xxh32_state *states,
                                                                uint64_t *frame_off)
@@ -483,15 +535,94 @@ __global__ void __launch_bounds__(128) frame_batch_tail_kernel(uint8_t *out, con
     uint64_t start, o;
     fb::frame_place(p, seg_off, &start, &o);
     for (uint32_t i = 0; i < p.hdr_len; i++) out[start + i] = p.hdr[i];
-    for (int b = 0; b < 4; b++) out[o + b] = 0;
-    o += 4;
-    if (states) {
+    if (p.hdr_len) {
+        for (int b = 0; b < 4; b++) out[o + b] = 0;
+        o += 4;
+    }
+    if (states && p.hdr_len) {
         const uint32_t h = fw::xxh32_digest(states[f]);
         for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(h >> (8 * b));
         o += 4;
     }
     frame_off[f] = start;
     if (f == n - 1) frame_off[n] = o;
+}
+
+// ---- sync-free batch frame encoder (lz4b200_frame_compress_batch_device_async) ------------------------------------------
+
+// Inclusive scan of v over the CTA's 1024 threads, saturating (fb::sat_add); `total` receives the sum of all 1024.  ws
+// is 32 shared words, free again when the scan returns.
+__device__ __forceinline__ uint64_t cta_scan_sat(uint64_t v, uint64_t *ws, uint64_t &total)
+{
+    uint64_t x = v;
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t y = __shfl_up_sync(kFull, x, d);
+        if ((threadIdx.x & 31) >= d) x = fb::sat_add(x, y);
+    }
+    if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = x;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        uint64_t t = ws[threadIdx.x];
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(kFull, t, d);
+            if (threadIdx.x >= d) t = fb::sat_add(t, y);
+        }
+        ws[threadIdx.x] = t;
+    }
+    __syncthreads();
+    const uint64_t r = threadIdx.x >= 32 ? fb::sat_add(ws[(threadIdx.x >> 5) - 1], x) : x;
+    total = ws[31];
+    __syncthreads();
+    return r;
+}
+
+// The device planner, one CTA over the frames in order, 1024 at a time.  Per frame: its plan and cost from d_in_off
+// and d_in_len (fb::batch_frame); the running sums of the costs decide the capacity rule (fb::capacity_status into
+// status[f]) and a frame past capacity is dropped (fb::drop_frame); the running sums of the frames' extents place it
+// (fb::place_frame), so a dropped frame sits where the frames inside end.  order[f] = f: the linked chains start in
+// index order.  *nb receives the blocks of the frames inside capacity.
+__global__ void __launch_bounds__(1024) frame_async_plan_kernel(const uint64_t *in_off, const uint64_t *in_len,
+                                                                uint32_t n, lz4b200_frame_info info,
+                                                                fb::BatchLimits lim, fb::FramePlan *plan,
+                                                                int32_t *status, uint32_t *order, uint32_t *nb)
+{
+    __shared__ uint64_t ws[32];
+    __shared__ fb::FrameCost carry;                // the costs of the frames of the chunks before
+    __shared__ fb::FramePlace placed;              // their extents
+    const uint32_t tail = info.content_checksum ? 8u : 4u;
+    if (threadIdx.x == 0) { carry = fb::FrameCost{0, 0, 0}; placed = fb::FramePlace{0, 0, 0}; }
+    __syncthreads();
+    for (uint32_t base = 0; base < n; base += 1024) {
+        const uint32_t f = base + threadIdx.x;
+        fb::FramePlan p{};
+        fb::FrameCost c{0, 0, 0}, incl, csum;
+        if (f < n) c = fb::batch_frame(p, info, in_off[f], in_len[f]);
+        incl.blocks = fb::sat_add(carry.blocks, cta_scan_sat(c.blocks, ws, csum.blocks));
+        incl.in_bytes = fb::sat_add(carry.in_bytes, cta_scan_sat(c.in_bytes, ws, csum.in_bytes));
+        incl.bound = fb::sat_add(carry.bound, cta_scan_sat(c.bound, ws, csum.bound));
+        const int32_t st = fb::capacity_status(incl, lim);
+        if (st != LZ4B200_OK) fb::drop_frame(p);
+        const fb::FramePlace e = f < n ? fb::frame_extent(p, tail) : fb::FramePlace{0, 0, 0};
+        fb::FramePlace before, esum;
+        before.blocks = placed.blocks + cta_scan_sat(e.blocks, ws, esum.blocks) - e.blocks;
+        before.slot = placed.slot + cta_scan_sat(e.slot, ws, esum.slot) - e.slot;
+        before.ovh = placed.ovh + cta_scan_sat(e.ovh, ws, esum.ovh) - e.ovh;
+        if (f < n) {
+            fb::place_frame(p, before);
+            plan[f] = p;
+            status[f] = st;
+            order[f] = f;
+        }
+        __syncthreads();                           // every thread has read carry and placed
+        if (threadIdx.x == 0) {
+            carry.blocks = fb::sat_add(carry.blocks, csum.blocks);
+            carry.in_bytes = fb::sat_add(carry.in_bytes, csum.in_bytes);
+            carry.bound = fb::sat_add(carry.bound, csum.bound);
+            placed.blocks += esum.blocks; placed.slot += esum.slot; placed.ovh += esum.ovh;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *nb = (uint32_t)placed.blocks;
 }
 
 // ---- batch frame decoder (lz4b200_frame_decompress_batch_device) --------------------------------------------------------
@@ -835,14 +966,6 @@ size_t block_size_bytes(int id)
     }
 }
 
-// BlockSize::from_buf_length — frame/header.rs:57-67
-int auto_block_size_id(size_t first_write_len)
-{
-    if (first_write_len > (256u << 10)) return 7;
-    if (first_write_len > (64u << 10)) return 5;
-    return 4;
-}
-
 // Device memory, freed with its owner on the owner's device.  reserve() grows with slack; resize() holds exactly n.
 template <typename T> struct DevBuf {
     T *p = nullptr;
@@ -1142,6 +1265,15 @@ lz4b200_status launch_decompress(lz4b200_ctx *ctx, const BatchArgs &args, cudaSt
     }
 }
 
+// u16 entries of one launch's global-table region: tables of 4096 for the CTAs per SM x chains per CTA that keep them
+// in global memory (none for the default shape, which keeps every table in shared memory).
+static size_t gtab_region_entries(const lz4b200_ctx *ctx)
+{
+    const int g16_m = (ctx->enc_g16 % 100) / 10, g16_g = ctx->enc_g16 >= 800 ? 8 : 16;
+    const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : ctx->enc_nib ? 8u * 7u : (size_t)kGtabCtasPerSm * (kGtabM - kGtabSmem));   // enc_nib: A/B build only
+    return (size_t)ctx->sm_count * chains_per_sm * 4096u;
+}
+
 // One table region per concurrently running launch (the host pipeline launches from up to 8 lanes): the ticket block
 // doubles as the region selector.
 static size_t table_slot(const lz4b200_ctx *ctx, const uint32_t *tickets)
@@ -1226,14 +1358,17 @@ static bool launch_compress_variant(lz4b200_ctx *ctx, const BatchArgs &a, uint32
 //                                                      tables in shared memory; lane-group matchers: more, global tables)
 //   fewer / dictionary                              -> shared-memory tables, matcher + emitter pairs
 //   blocks > 64 KiB without dictionary              -> one chain per CTA over the TMA-fed ring when enabled
+// `gtab` is the region of gtab_region_entries(ctx) u16 entries the global-table shapes keep their tables in; null: the
+// context's region for `tickets` (one per concurrently running launch).  A caller whose tickets are not the context's
+// passes its own region, and then runs the product kernels only.
 lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t max_in_len, cudaStream_t s,
-                               uint32_t *tickets = nullptr)
+                               uint32_t *tickets = nullptr, uint16_t *gtab = nullptr)
 {
     if (!tickets) tickets = ctx->d_tickets.p;
     if (args.nblocks == 0) return LZ4B200_OK;
     const BatchArgs &a = args;
 #ifdef LZ4B200_AB_VARIANTS
-    {
+    if (!gtab) {
         lz4b200_status vst;
         if (launch_compress_variant(ctx, a, max_in_len, s, tickets, &vst)) return vst;
     }
@@ -1247,13 +1382,12 @@ lz4b200_status launch_compress(lz4b200_ctx *ctx, const BatchArgs &args, uint32_t
     }
     {                                                       // u16 tables: every block with input (+ dictionary) <= 64 KiB
         if (!a.dict_len && a.nblocks > (uint32_t)ctx->sm_count * 24u) {
-            // u16 entries: tables of 4096 for the CTAs per SM x chains per CTA that keep them in global memory, one region
-            // per concurrently running launch
-            const int g16_m = (ctx->enc_g16 % 100) / 10, g16_g = ctx->enc_g16 >= 800 ? 8 : 16;
-            const size_t chains_per_sm = ctx->enc_g16 ? (size_t)ctx->enc_g16_ctas * (32 / g16_g) * g16_m : (ctx->enc_nib >= 4 ? 112u : ctx->enc_nib ? 8u * 7u : (size_t)kGtabCtasPerSm * (kGtabM - kGtabSmem));   // enc_nib: A/B build only
-            const size_t region = (size_t)ctx->sm_count * chains_per_sm * 4096u;
-            if (!ctx->check(ctx->d_gtab16.reserve(region * 9u), "gtab")) return LZ4B200_CUDA_ERROR;
-            uint16_t *gt = ctx->d_gtab16.p + table_slot(ctx, tickets) * region;
+            uint16_t *gt = gtab;
+            if (!gt) {
+                const size_t region = gtab_region_entries(ctx);
+                if (!ctx->check(ctx->d_gtab16.reserve(region * 9u), "gtab")) return LZ4B200_CUDA_ERROR;
+                gt = ctx->d_gtab16.p + table_slot(ctx, tickets) * region;
+            }
 #ifdef LZ4B200_AB_VARIANTS
             if (ctx->enc_nib && !ctx->enc_g16) {                                     // tags in shared memory: 1 = nibbles x 8 CTAs, 2 = bytes x 6 CTAs, 3 = nibbles x 6 CTAs (40 registers)
                 const uint32_t ctas = std::min(ctx->enc_nib_ctas, ctx->enc_nib == 1 ? 8 : 6);
@@ -2263,23 +2397,7 @@ lz4b200_status lz4b200_decompress_size_prepended(lz4b200_ctx *ctx, const uint8_t
 
 size_t lz4b200_frame_write_header(const lz4b200_frame_info *info, uint8_t *out, size_t cap)
 {
-    // FrameInfo::write — frame/header.rs:232-275
-    uint8_t buf[19];
-    size_t o = 0;
-    wr32(buf, 0x184D2204u); o = 4;
-    uint8_t flg = 0x40;
-    if (info->block_checksums) flg |= 0x10;
-    if (info->content_checksum) flg |= 0x04;
-    if (!info->linked) flg |= 0x20;
-    if (info->has_content_size) flg |= 0x08;
-    buf[o++] = flg;
-    buf[o++] = (uint8_t)(info->block_size_id << 4);
-    if (info->has_content_size) { memcpy(buf + o, &info->content_size, 8); o += 8; }
-    buf[o] = (uint8_t)(lz4b200_xxh32(buf + 4, o - 4, 0) >> 8);
-    o++;
-    if (cap < o) return 0;
-    memcpy(out, buf, o);
-    return o;
+    return fb::write_header(*info, out, cap);
 }
 
 size_t lz4b200_frame_blocks_bound(size_t in_len, size_t block_size)
@@ -2293,38 +2411,106 @@ size_t lz4b200_frame_bound(size_t n, const lz4b200_frame_info *info)
     int id = info && info->block_size_id ? info->block_size_id : 4;
     size_t bs = block_size_bytes(id);
     if (!bs) bs = 64u << 10;
-    size_t nb = (n + bs - 1) / bs;
-    return 19 + n + nb * 8 + 8;
+    return fb::frame_bound_bytes(n, bs);
 }
 
 }  // extern "C"
 
 namespace {
 
-// Sets what `info` (block size resolved) and the input d_in[in_off, in_off + in_len) decide of the zeroed plan p, the
-// header included; fb::plan_frame places it after the frame before.  p is filled in place, not returned: copying a
-// returned plan into the batch's table stalls the host on every frame.
-void frame_plan(fb::FramePlan &p, const lz4b200_frame_info &info, uint64_t in_off, uint64_t in_len)
+// The device buffers of the frame encoders' pipeline.  The synchronous calls take them from the context's reserved
+// buffers, the sync-free call carves them from the caller's scratch (CompressScratch).  Per frame: the plans, the
+// linked frames' order and the content hashes; per block: the compressor's arguments and results, the segment sizes,
+// their scan and the packed destinations; the scratch slots; the encoders' ticket words and table region (null: the
+// context's).  With nb_dev the batch's block count is only known on the device: the per-block launches are sized by
+// the capacity the host passes, and their threads past *nb_dev write nothing the output depends on.
+struct FrameBufs {
+    fb::FramePlan *plan;
+    uint32_t *order;
+    lz4b200_xxh32_state *content;
+    uint64_t *in_off, *out_off, *seg_off, *gdst;
+    uint32_t *in_len, *out_cap, *out_len, *info, *seg_size, *payload_len;
+    int32_t *status;
+    uint8_t *flags, *pick, *slots;
+    uint32_t *tickets;
+    uint16_t *gtab;
+    const uint32_t *nb_dev;
+};
+
+// The launches of every frame encoder, over n >= 1 frames whose plans are at m.plan on the device and nb blocks (or
+// *m.nb_dev of them, at most nb): one thread per block writes the compressor's arguments, one launch compresses every
+// block of every frame, the segment sizes (with room for a checksum after each payload when `block_checksums`) are
+// scanned, one gather packs every [BlockInfo | payload] at its frame's place, and one thread per block writes the
+// block checksums.  max_in_len is launch_compress's bound on the blocks' lengths.  A device position d_pos_in moves
+// every block *d_pos_in bytes further, and *d_pos_out receives the end of the blocks.  With `content_checksum` one CTA
+// per frame hashes its content; with d_frame_off one thread per frame writes its header, EndMark, digest (when hashed)
+// and d_frame_off[f], and d_frame_off[n] the total.  With `linked` the frames are BlockMode::Linked: one launch of
+// lz4_compress_frames_linked runs one chain per frame, taking frames in m.order, in place of launch_compress, and
+// everything else is the same.
+lz4b200_status enqueue_frames(lz4b200_ctx *ctx, const FrameBufs &m, const uint8_t *d_in, uint32_t n, uint32_t nb,
+                              uint32_t max_in_len, bool block_checksums, bool content_checksum, uint8_t *d_out,
+                              uint64_t *d_frame_off, const uint64_t *d_pos_in, uint64_t *d_pos_out, cudaStream_t s,
+                              bool linked)
 {
-    p.in_off = in_off;
-    p.in_len = in_len;
-    p.bs = (uint32_t)block_size_bytes(info.block_size_id);
-    p.fresh = fb::fresh_period(p.bs);
-    p.hdr_len = (uint8_t)lz4b200_frame_write_header(&info, p.hdr, sizeof p.hdr);
+    const uint32_t bgrid = (nb + 127) / 128;
+    if (nb) {
+        frame_batch_blocks_kernel<<<bgrid, 128, 0, s>>>(m.plan, n, nb, m.in_off, m.in_len, m.out_off, m.out_cap, m.flags,
+                                                        m.gdst, m.nb_dev);
+        CTX_CUDA(ctx, cudaGetLastError());
+        BatchArgs a{d_in, m.in_off, m.in_len, m.flags, m.slots, m.out_off, m.out_cap, m.out_len, m.status, nullptr, nb,
+                    nullptr};
+        if (linked) {
+            const uint32_t grid = std::min<uint32_t>((n + kLinkedPairs - 1) / kLinkedPairs,
+                                                     (uint32_t)(ctx->sm_count * ctx->enc_linked_ctas_per_sm));
+            lz4_compress_frames_linked<<<grid, kLinkedPairs * 64, linked_smem_bytes(), s>>>(a, m.plan, m.order, n,
+                                                                                           m.tickets + 6);
+            ctx->last_kernel[0] = "lz4_compress_frames_linked";
+            CTX_CUDA(ctx, cudaGetLastError());
+        } else {
+            const lz4b200_status st = launch_compress(ctx, a, max_in_len, s, m.tickets, m.gtab);
+            if (st != LZ4B200_OK) return st;
+        }
+        if (m.nb_dev)
+            frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(m.out_len, m.in_len, nb, block_checksums ? 4u : 0u,
+                                                                    m.info, m.pick, m.seg_size, m.payload_len, m.nb_dev);
+        else
+            frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(m.out_len, m.in_len, nb, block_checksums ? 4u : 0u,
+                                                                    m.info, m.pick, m.seg_size, m.payload_len);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    if (m.nb_dev) scan_sizes_kernel<<<1, 1024, 0, s>>>(m.seg_size, m.seg_off, nb, m.nb_dev);
+    else scan_sizes_kernel<<<1, 1024, 0, s>>>(m.seg_size, m.seg_off, nb);        // no blocks: seg_off[0] = 0
+    CTX_CUDA(ctx, cudaGetLastError());
+    if (nb) {
+        frame_batch_dst_kernel<<<bgrid, 128, 0, s>>>(m.seg_off, nb, m.gdst, d_pos_in, d_pos_out, m.nb_dev);
+        GatherArgs g{m.slots, d_in, m.out_off, m.in_off, m.payload_len, m.payload_len, m.pick, m.info, d_out, m.gdst, nb};
+        const uint32_t ggrid = std::min<uint32_t>(std::max<uint32_t>(nb, (uint32_t)ctx->sm_count * 2),
+                                                  (uint32_t)ctx->sm_count * 8);
+        if (m.nb_dev) gather_segments_kernel<<<ggrid, 256, 0, s>>>(g, m.nb_dev);
+        else gather_segments_kernel<<<ggrid, 256, 0, s>>>(g);
+        CTX_CUDA(ctx, cudaGetLastError());
+        if (block_checksums) {
+            frame_block_checksum_kernel<<<bgrid, 128, 0, s>>>(d_out, m.gdst, m.payload_len, nb, m.nb_dev);
+            CTX_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    if (content_checksum) {
+        frame_batch_content_kernel<<<n, 256, 0, s>>>(d_in, m.plan, m.content);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    if (d_frame_off) {
+        frame_batch_tail_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_out, m.plan, n, m.seg_off,
+                                                                content_checksum ? m.content : nullptr, d_frame_off);
+        CTX_CUDA(ctx, cudaGetLastError());
+    }
+    return LZ4B200_OK;
 }
 
-// The pipeline of every frame encoder: enqueues the n >= 1 frames of plan (placed by fb::plan_frame) on `s`.  One plan
-// reaches the device as a kernel argument, more with one copy from pageable memory, which cudaMemcpyAsync stages before
-// it returns, so back-to-back calls never share a host buffer.  Then one thread per block writes the compressor's
-// arguments, one launch compresses every block of every frame, the segment sizes (with room for a checksum after each
-// payload when `block_checksums`) are scanned, one gather packs every [BlockInfo | payload] at its frame's place, and
-// one thread per block writes the block checksums.  max_in_len is launch_compress's bound on the blocks' lengths.  A
-// device position d_pos_in moves every block *d_pos_in bytes further, and *d_pos_out receives the end of the blocks.
-// With `content_checksum` one CTA per frame hashes its content; with d_frame_off one thread per frame writes its
-// header, EndMark, digest (when hashed) and d_frame_off[f], and d_frame_off[n] the total.
-// With `linked_order` (a host array of n frame indices, longest frame first) the frames are BlockMode::Linked: one
-// launch of lz4_compress_frames_linked runs one chain per frame, taking frames in that order, in place of
-// launch_compress, and everything else is the same.
+// The pipeline of every synchronous frame encoder: enqueues the n >= 1 frames of plan (placed by fb::plan_frame) on
+// `s` through enqueue_frames, over the context's buffers.  One plan reaches the device as a kernel argument, more with
+// one copy from pageable memory, which cudaMemcpyAsync stages before it returns, so back-to-back calls never share a
+// host buffer.  With `linked_order` (a host array of n frame indices, longest frame first) the frames are
+// BlockMode::Linked and their chains start in that order.
 lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::FramePlan *plan, uint32_t n,
                                uint32_t max_in_len, bool block_checksums, bool content_checksum, uint8_t *d_out,
                                uint64_t *d_frame_off, const uint64_t *d_pos_in, uint64_t *d_pos_out, cudaStream_t s,
@@ -2348,59 +2534,16 @@ lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::
     } else {
         CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_fplan.p, plan, n * sizeof(fb::FramePlan), cudaMemcpyHostToDevice, s));
     }
-
-    const uint32_t bgrid = (nb + 127) / 128;
-    if (nb) {
-        frame_batch_blocks_kernel<<<bgrid, 128, 0, s>>>(ctx->d_fplan.p, n, nb, ctx->d_in_off.p, ctx->d_in_len.p,
-                                                        ctx->d_out_off.p, ctx->d_out_cap.p, ctx->d_flags.p,
-                                                        ctx->d_gdst.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-        BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
-                    ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
-        if (linked_order) {
-            CTX_CUDA(ctx, ctx->d_forder.reserve(n));
-            CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_forder.p, linked_order, n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-            const uint32_t grid = std::min<uint32_t>((n + kLinkedPairs - 1) / kLinkedPairs,
-                                                     (uint32_t)(ctx->sm_count * ctx->enc_linked_ctas_per_sm));
-            lz4_compress_frames_linked<<<grid, kLinkedPairs * 64, linked_smem_bytes(), s>>>(a, ctx->d_fplan.p,
-                                                                                           ctx->d_forder.p, n,
-                                                                                           ctx->d_tickets.p + 6);
-            ctx->last_kernel[0] = "lz4_compress_frames_linked";
-            CTX_CUDA(ctx, cudaGetLastError());
-        } else {
-            const lz4b200_status st = launch_compress(ctx, a, max_in_len, s);
-            if (st != LZ4B200_OK) return st;
-        }
-        frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb,
-                                                                block_checksums ? 4u : 0u, ctx->d_info.p,
-                                                                ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
-        CTX_CUDA(ctx, cudaGetLastError());
+    if (linked_order && nb) {
+        CTX_CUDA(ctx, ctx->d_forder.reserve(n));
+        CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_forder.p, linked_order, n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     }
-    scan_sizes_kernel<<<1, 1024, 0, s>>>(ctx->d_seg_size.p, ctx->d_seg_off.p, nb);   // nb == 0: seg_off[0] = 0
-    CTX_CUDA(ctx, cudaGetLastError());
-    if (nb) {
-        frame_batch_dst_kernel<<<bgrid, 128, 0, s>>>(ctx->d_seg_off.p, nb, ctx->d_gdst.p, d_pos_in, d_pos_out);
-        GatherArgs g{ctx->d_slots.p, d_in, ctx->d_out_off.p, ctx->d_in_off.p, ctx->d_payload_len.p, ctx->d_payload_len.p,
-                     ctx->d_pick.p, ctx->d_info.p, d_out, ctx->d_gdst.p, nb};
-        gather_segments_kernel<<<std::min<uint32_t>(std::max<uint32_t>(nb, (uint32_t)ctx->sm_count * 2),
-                                                    (uint32_t)ctx->sm_count * 8), 256, 0, s>>>(g);
-        CTX_CUDA(ctx, cudaGetLastError());
-        if (block_checksums) {
-            frame_block_checksum_kernel<<<bgrid, 128, 0, s>>>(d_out, ctx->d_gdst.p, ctx->d_payload_len.p, nb);
-            CTX_CUDA(ctx, cudaGetLastError());
-        }
-    }
-    if (content_checksum) {
-        frame_batch_content_kernel<<<n, 256, 0, s>>>(d_in, ctx->d_fplan.p, ctx->d_content.p);
-        CTX_CUDA(ctx, cudaGetLastError());
-    }
-    if (d_frame_off) {
-        frame_batch_tail_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_out, ctx->d_fplan.p, n, ctx->d_seg_off.p,
-                                                                content_checksum ? ctx->d_content.p : nullptr,
-                                                                d_frame_off);
-        CTX_CUDA(ctx, cudaGetLastError());
-    }
-    return LZ4B200_OK;
+    const FrameBufs m{ctx->d_fplan.p, ctx->d_forder.p, ctx->d_content.p, ctx->d_in_off.p, ctx->d_out_off.p,
+                      ctx->d_seg_off.p, ctx->d_gdst.p, ctx->d_in_len.p, ctx->d_out_cap.p, ctx->d_out_len.p,
+                      ctx->d_info.p, ctx->d_seg_size.p, ctx->d_payload_len.p, ctx->d_status.p, ctx->d_flags.p,
+                      ctx->d_pick.p, ctx->d_slots.p, ctx->d_tickets.p, nullptr, nullptr};
+    return enqueue_frames(ctx, m, d_in, n, nb, max_in_len, block_checksums, content_checksum, d_out, d_frame_off,
+                          d_pos_in, d_pos_out, s, linked_order != nullptr);
 }
 
 }  // namespace
@@ -2534,7 +2677,7 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
     *written = 0;
     lz4b200_frame_info info = *info_in;
     if (info.linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
-    if (info.block_size_id == 0) info.block_size_id = auto_block_size_id(first_write_len);   // compress.rs:236-238
+    if (info.block_size_id == 0) info.block_size_id = fb::auto_block_size_id(first_write_len);   // compress.rs:236-238
     if (info.block_size_id < 4 || info.block_size_id > 7) return LZ4B200_INVALID_ARGUMENT;
     if (info.has_content_size && info.content_size != n) return LZ4B200_FRAME_CONTENT_LENGTH; // compress.rs:212-219
     if (cap < lz4b200_frame_bound(n, &info)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
@@ -2542,7 +2685,7 @@ lz4b200_status lz4b200_frame_compress(lz4b200_ctx *ctx, const uint8_t *in, size_
     cudaStream_t s = ctx->stream;
 
     fb::FramePlan plan{};
-    frame_plan(plan, info, 0, n);
+    fb::frame_plan(plan, info, 0, n);
     CTX_CUDA(ctx, ctx->d_in.reserve(n + 16));
     CTX_CUDA(ctx, ctx->d_out.reserve(lz4b200_frame_bound(n, &info)));
     CTX_CUDA(ctx, ctx->d_off_b.reserve(2));
@@ -2569,7 +2712,7 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
     if (!ctx || !info_in || !d_out || !d_written || (!d_in && n)) return LZ4B200_INVALID_ARGUMENT;
     lz4b200_frame_info info = *info_in;
     if (info.linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
-    if (info.block_size_id == 0) info.block_size_id = auto_block_size_id(first_write_len);   // compress.rs:236-238
+    if (info.block_size_id == 0) info.block_size_id = fb::auto_block_size_id(first_write_len);   // compress.rs:236-238
     if (info.block_size_id < 4 || info.block_size_id > 7) return LZ4B200_INVALID_ARGUMENT;
     if (info.has_content_size && info.content_size != n) return LZ4B200_FRAME_CONTENT_LENGTH; // compress.rs:212-219
     if (cap < lz4b200_frame_bound(n, &info)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
@@ -2577,7 +2720,7 @@ lz4b200_status lz4b200_frame_compress_device(lz4b200_ctx *ctx, const uint8_t *d_
     cudaStream_t s = (cudaStream_t)stream;
 
     fb::FramePlan plan{};
-    frame_plan(plan, info, 0, n);
+    fb::frame_plan(plan, info, 0, n);
     CTX_CUDA(ctx, ctx->d_off_b.reserve(2));
     const lz4b200_status st = compress_frames(ctx, d_in, &plan, 1, (uint32_t)std::min<uint64_t>(n, plan.bs),
                                               info.block_checksums, info.content_checksum, d_out, ctx->d_off_b.p,
@@ -2612,10 +2755,10 @@ lz4b200_status compress_frame_batch(lz4b200_ctx *ctx, const uint8_t *d_in, const
     bool small = false;                                     // some block has at most 64 KiB
     for (size_t f = 0; f < nframes; f++) {
         lz4b200_frame_info fi = *info;
-        if (id == 0) fi.block_size_id = auto_block_size_id(in_len[f]);                      // compress.rs:236-238
+        if (id == 0) fi.block_size_id = fb::auto_block_size_id(in_len[f]);                      // compress.rs:236-238
         fi.content_size = in_len[f];
         fb::FramePlan &p = plan[f];
-        frame_plan(p, fi, in_off[f], in_len[f]);
+        fb::frame_plan(p, fi, in_off[f], in_len[f]);
         const uint64_t nb = fb::frame_blocks(p);
         if (nblocks + nb > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
         fb::plan_frame(p, f ? &plan[f - 1] : nullptr, tail);
@@ -2668,6 +2811,126 @@ lz4b200_status lz4b200_frame_compress_linked_batch_device(lz4b200_ctx *ctx, cons
                                                           void *stream)
 {
     return compress_frame_batch(ctx, d_in, in_off, in_len, info, d_out, out_cap, d_frame_off, nframes, stream, true);
+}
+
+}  // extern "C"
+
+// ---- sync-free batch frame encoder ---------------------------------------------------------------------------------------
+namespace {
+
+// Slot bytes that hold the blocks of any batch of at most `cap` blocks and `in_bytes` input bytes: a block of len bytes
+// takes fb::slot_bytes_for(len) <= 35 + len x 110 / 100, and 16 bytes of slack follow, as the synchronous call
+// reserves.  SIZE_MAX past any device's memory.
+size_t async_slot_bytes(size_t cap, size_t in_bytes)
+{
+    if (in_bytes >> 60) return SIZE_MAX;
+    return in_bytes / 100 * 110 + in_bytes % 100 * 110 / 100 + 35 * cap + 16;
+}
+
+// The caller's scratch of lz4b200_frame_compress_batch_device_async, carved into 256-byte aligned arrays: per frame
+// (n) the plans, the linked order and the content hashes; per block (cap) the pipeline's arrays; the slots; the
+// encoder's global-table region (gtab u16 entries, none for the default shape); the ticket words and the device block
+// count.  With a null base only `bytes` is meaningful.
+struct CompressScratch {
+    FrameBufs m{};
+    uint32_t *nb = nullptr;
+    size_t bytes = 0;
+
+    CompressScratch(void *base, size_t n, size_t cap, size_t slot_bytes, size_t gtab)
+    {
+        auto take = [&](auto *&p, size_t count) {
+            p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + bytes);
+            bytes += (count * sizeof(*p) + 255) & ~size_t(255);
+        };
+        take(m.plan, n); take(m.order, n); take(m.content, n);
+        take(m.in_off, cap); take(m.out_off, cap); take(m.seg_off, cap + 1); take(m.gdst, cap);
+        take(m.in_len, cap); take(m.out_cap, cap); take(m.out_len, cap); take(m.info, cap); take(m.seg_size, cap);
+        take(m.payload_len, cap); take(m.status, cap); take(m.flags, cap); take(m.pick, cap);
+        take(m.slots, slot_bytes); take(m.gtab, gtab); take(m.tickets, 8); take(nb, 1);
+        m.nb_dev = nb;
+    }
+};
+
+// u16 entries of the global-table region a launch over cap blocks needs (launch_compress takes the global-table shapes
+// above 24 blocks per SM).
+size_t async_gtab_entries(const lz4b200_ctx *ctx, size_t cap)
+{
+    return cap > (size_t)ctx->sm_count * 24u ? gtab_region_entries(ctx) : 0;
+}
+
+// lz4b200_frame_compress_batch_device_async and its linked form: argument checks, the ticket reset, the device planner,
+// then the frame encoders' launches over the scratch, sized by nframes and max_blocks.
+lz4b200_status compress_frame_batch_async(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
+                                          const uint64_t *d_in_len, const lz4b200_frame_info *info, uint8_t *d_out,
+                                          size_t out_cap, uint64_t *d_frame_off, int32_t *d_status, size_t nframes,
+                                          size_t max_blocks, size_t max_in_bytes, void *d_scratch,
+                                          size_t scratch_bytes, void *stream, bool linked)
+{
+    if (!ctx || !info || !d_frame_off) return LZ4B200_INVALID_ARGUMENT;
+    if (nframes && (!d_in || !d_in_off || !d_in_len || (!d_out && out_cap) || !d_status || !d_scratch))
+        return LZ4B200_INVALID_ARGUMENT;
+    if (nframes > 0xffffffffull || max_blocks > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    const int id = info->block_size_id;
+    if (id != 0 && (id < 4 || id > 7)) return LZ4B200_INVALID_ARGUMENT;
+    if (!linked && info->linked) return LZ4B200_FRAME_LINKED_UNSUPPORTED;
+    if (linked && !info->linked) return LZ4B200_INVALID_ARGUMENT;
+    if (scratch_bytes < lz4b200_frame_compress_batch_device_async_scratch(ctx, nframes, max_blocks, max_in_bytes))
+        return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (nframes == 0) {
+        CTX_CUDA(ctx, cudaMemsetAsync(d_frame_off, 0, 8, s));
+        return LZ4B200_OK;
+    }
+    const uint32_t n = (uint32_t)nframes, cap = (uint32_t)max_blocks;
+    CompressScratch m(d_scratch, n, cap, async_slot_bytes(cap, max_in_bytes), async_gtab_entries(ctx, cap));
+    CTX_CUDA(ctx, cudaMemsetAsync(m.m.tickets, 0, 8 * sizeof(uint32_t), s));
+    frame_async_plan_kernel<<<1, 1024, 0, s>>>(d_in_off, d_in_len, n, *info,
+                                               fb::BatchLimits{max_blocks, max_in_bytes, out_cap}, m.m.plan, d_status,
+                                               m.m.order, m.nb);
+    CTX_CUDA(ctx, cudaGetLastError());
+    // the block lengths stay on the device: a fixed 64 KiB block size bounds them, any other size or Auto runs both
+    // table widths
+    const uint32_t max_in_len = id == 4 ? 65536u : 0u;
+    return enqueue_frames(ctx, m.m, d_in, n, cap, max_in_len, info->block_checksums, info->content_checksum, d_out,
+                          d_frame_off, nullptr, nullptr, s, linked);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t lz4b200_frame_compress_batch_device_async_scratch(const lz4b200_ctx *ctx, size_t nframes, size_t max_blocks,
+                                                         size_t max_in_bytes)
+{
+    if (nframes > 0xffffffffull || max_blocks > 0xffffffffull || !ctx) return SIZE_MAX;
+    if (!nframes) return 0;
+    const size_t slots = async_slot_bytes(max_blocks, max_in_bytes);
+    if (slots == SIZE_MAX) return SIZE_MAX;
+    return CompressScratch(nullptr, nframes, max_blocks, slots, async_gtab_entries(ctx, max_blocks)).bytes;
+}
+
+lz4b200_status lz4b200_frame_compress_batch_device_async(lz4b200_ctx *ctx, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                         const uint64_t *d_in_len, const lz4b200_frame_info *info,
+                                                         uint8_t *d_out, size_t out_cap, uint64_t *d_frame_off,
+                                                         int32_t *d_status, size_t nframes, size_t max_blocks,
+                                                         size_t max_in_bytes, void *d_scratch, size_t scratch_bytes,
+                                                         void *stream)
+{
+    return compress_frame_batch_async(ctx, d_in, d_in_off, d_in_len, info, d_out, out_cap, d_frame_off, d_status,
+                                      nframes, max_blocks, max_in_bytes, d_scratch, scratch_bytes, stream, false);
+}
+
+lz4b200_status lz4b200_frame_compress_linked_batch_device_async(lz4b200_ctx *ctx, const uint8_t *d_in,
+                                                                const uint64_t *d_in_off, const uint64_t *d_in_len,
+                                                                const lz4b200_frame_info *info, uint8_t *d_out,
+                                                                size_t out_cap, uint64_t *d_frame_off,
+                                                                int32_t *d_status, size_t nframes, size_t max_blocks,
+                                                                size_t max_in_bytes, void *d_scratch,
+                                                                size_t scratch_bytes, void *stream)
+{
+    return compress_frame_batch_async(ctx, d_in, d_in_off, d_in_len, info, d_out, out_cap, d_frame_off, d_status,
+                                      nframes, max_blocks, max_in_bytes, d_scratch, scratch_bytes, stream, true);
 }
 
 namespace {

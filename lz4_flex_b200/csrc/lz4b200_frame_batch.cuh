@@ -7,7 +7,10 @@
 // where its [BlockInfo | payload (| checksum)] segment lands in the packed output (batch_block).  Frames lie back to
 // back: frame f starts at seg_off[first_block] + ovh, where seg_off is the exclusive scan of every block's segment size
 // and ovh the header, EndMark and digest bytes of the frames before it (frame_place).
-// The header also compiles for the host alone (tests/cpp/frame_batch_host.cpp) for the CPU tests.
+// The sync-free batch call plans its frames on the device instead (batch_frame, capacity_status, frame_extent and
+// place_frame in one CTA's scan), from the same functions.
+// The header also compiles for the host alone (tests/cpp/frame_batch_host.cpp, frame_batch_async_host.cpp) for the CPU
+// tests.
 #pragma once
 #include "lz4b200_frame_walk.cuh"
 
@@ -104,6 +107,123 @@ FW_FN void frame_place(const FramePlan &p, const uint64_t *seg_off, uint64_t *st
 {
     *start = seg_off[p.first_block] + p.ovh;
     *endmark = seg_off[p.first_block + frame_blocks(p)] + p.ovh + p.hdr_len;
+}
+
+// ---- the header, shared by the host entry points and the device planner ------------------------------------------------
+
+// BlockSize::from_buf_length — frame/header.rs:57-67
+FW_FN int auto_block_size_id(uint64_t first_write_len)
+{
+    if (first_write_len > (256u << 10)) return 7;
+    if (first_write_len > (64u << 10)) return 5;
+    return 4;
+}
+
+// FrameInfo::write — frame/header.rs:232-275: the header's bytes at out, their count (at most 15), or 0 when cap cannot
+// hold them.
+FW_FN uint32_t write_header(const lz4b200_frame_info &info, uint8_t *out, uint64_t cap)
+{
+    uint8_t buf[15] = {0x04, 0x22, 0x4D, 0x18};
+    uint32_t o = 4;
+    uint8_t flg = 0x40;
+    if (info.block_checksums) flg |= 0x10;
+    if (info.content_checksum) flg |= 0x04;
+    if (!info.linked) flg |= 0x20;
+    if (info.has_content_size) flg |= 0x08;
+    buf[o++] = flg;
+    buf[o++] = (uint8_t)(info.block_size_id << 4);
+    if (info.has_content_size)
+        for (int i = 0; i < 8; i++) buf[o++] = (uint8_t)(info.content_size >> (8 * i));
+    buf[o] = (uint8_t)(fw::xxh32(buf + 4, o - 4, 0) >> 8);
+    o++;
+    if (cap < o) return 0;
+    for (uint32_t i = 0; i < o; i++) out[i] = buf[i];
+    return o;
+}
+
+// lz4b200_frame_bound for n input bytes in blocks of bs: the header at its longest, every block's BlockInfo and
+// checksum, the EndMark and the digest.
+FW_FN uint64_t frame_bound_bytes(uint64_t n, uint64_t bs) { return 19 + n + (n + bs - 1) / bs * 8 + 8; }
+
+// Sets what `info` (block size resolved) and the input d_in[in_off, in_off + in_len) decide of the zeroed plan p, the
+// header included; plan_frame places it after the frame before.  p is filled in place, not returned: copying a
+// returned plan into the batch's table stalls the host on every frame.
+FW_FN void frame_plan(FramePlan &p, const lz4b200_frame_info &info, uint64_t in_off, uint64_t in_len)
+{
+    p.in_off = in_off;
+    p.in_len = in_len;
+    p.bs = (uint32_t)fw::block_size_bytes(info.block_size_id);
+    p.fresh = fresh_period(p.bs);
+    p.hdr_len = (uint8_t)write_header(info, p.hdr, sizeof p.hdr);
+}
+
+// ---- the sync-free batch planner (lz4b200_frame_compress_batch_device_async) -------------------------------------------
+// One CTA scans the frames on the device.  Frame f is planned only if frames 0..f together fit the three limits; since
+// every frame adds a non-negative amount to each sum, the frames inside form a prefix.  A frame past them keeps its
+// place but has no input and no header (in_len = 0, hdr_len = 0): no blocks, and nothing of it is written.
+
+// Saturating: a sum that would wrap stays past every limit.
+FW_FN uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ull : a + b; }
+
+struct BatchLimits {
+    uint64_t blocks, in_bytes, out_bytes;   // max_blocks, max_in_bytes, out_cap
+};
+
+// What one frame adds to the sums the capacity rule checks.
+struct FrameCost {
+    uint64_t blocks, in_bytes, bound;       // blocks, input bytes, lz4b200_frame_bound bytes
+};
+
+// Frame f of the batch, before placement: its plan under *info (Auto resolved from in_len, the content size in_len) and
+// its cost.  A frame of 2^62 bytes or more has more than 2^32 blocks, past every capacity: its cost is taken at 2^62
+// bytes, so that no sum wraps.
+FW_FN FrameCost batch_frame(FramePlan &p, const lz4b200_frame_info &info, uint64_t in_off, uint64_t in_len)
+{
+    lz4b200_frame_info fi = info;
+    if (fi.block_size_id == 0) fi.block_size_id = auto_block_size_id(in_len);                  // compress.rs:236-238
+    fi.content_size = in_len;
+    frame_plan(p, fi, in_off, in_len);
+    const uint64_t n = in_len < (1ull << 62) ? in_len : (1ull << 62);
+    FrameCost c;
+    c.blocks = (n + p.bs - 1) / p.bs;
+    c.in_bytes = n;
+    c.bound = frame_bound_bytes(n, p.bs);
+    return c;
+}
+
+// The status of a frame whose frames 0..f sum to `incl`: OK inside all three limits; else the first limit passed, in
+// the order blocks, input bytes, bound, decides: INVALID_ARGUMENT for the first two, COMPRESS_OUTPUT_TOO_SMALL for the
+// bound.
+FW_FN int32_t capacity_status(const FrameCost &incl, const BatchLimits &lim)
+{
+    if (incl.blocks > lim.blocks || incl.in_bytes > lim.in_bytes) return LZ4B200_INVALID_ARGUMENT;
+    if (incl.bound > lim.out_bytes) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
+    return LZ4B200_OK;
+}
+
+// A frame past capacity: no blocks, no header.
+FW_FN void drop_frame(FramePlan &p) { p.in_len = 0; p.hdr_len = 0; }
+
+// What frame p adds to the places of the frames after it (plan_frame's sums): its blocks, its scratch and its header,
+// EndMark and digest bytes.  A dropped frame adds nothing.
+struct FramePlace {
+    uint64_t blocks, slot, ovh;
+};
+FW_FN FramePlace frame_extent(const FramePlan &p, uint32_t tail_len)
+{
+    FramePlace e;
+    e.blocks = frame_blocks(p);
+    e.slot = frame_slot_bytes(p);
+    e.ovh = p.hdr_len ? p.hdr_len + tail_len : 0u;
+    return e;
+}
+
+// Places p after frames whose extents sum to `before`.
+FW_FN void place_frame(FramePlan &p, const FramePlace &before)
+{
+    p.first_block = (uint32_t)before.blocks;
+    p.slot_base = before.slot;
+    p.ovh = before.ovh;
 }
 
 }  // namespace fb

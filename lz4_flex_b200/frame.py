@@ -480,6 +480,112 @@ def decompress_frames_device_async(d_in, offsets, lengths, out, out_offsets, out
     return DecodedFrames(out, oo, results)
 
 
+@dataclass
+class CompressedFrames:
+    """What compress_frames_device_async() returns, device tensors valid once the stream has reached the call: `out`,
+    the int64 frame_offsets (nframes + 1 entries: frame i is out[frame_offsets[i]:frame_offsets[i + 1]]) and the int32
+    statuses, one per frame: 0 for a frame compressed, LZ4B200_INVALID_ARGUMENT (200) or
+    LZ4B200_COMPRESS_OUTPUT_TOO_SMALL (1) for a frame past capacity."""
+    out: "object"
+    frame_offsets: "object"
+    statuses: "object"
+
+
+def default_compress_max_blocks(in_bytes: int, nframes: int) -> int:
+    """The block capacity compress_frames_device_async() assumes when none is given: in_bytes // 65536 + nframes.
+    Every block of a frame but its last holds a full block of at least 64 KiB, so frames that do not overlap in d_in
+    and hold in_bytes bytes together have at most in_bytes // 65536 + nframes blocks."""
+    return in_bytes // 65536 + nframes
+
+
+def compress_out_cap(nframes: int, max_in_bytes: int, frame_info: FrameInfo | None = None) -> int:
+    """An out_cap that holds every batch of at most nframes frames and max_in_bytes input bytes under frame_info, so that
+    a frame within the other two limits of compress_frames_device_async() never fails on out_cap: 27 F + T + 8 (ceil(T /
+    bs) + F) for F frames of T bytes, bs the fixed block size or, for Auto, 64 KiB (the smallest Auto picks).  Every
+    frame's lz4b200_frame_bound is 27 + n + 8 ceil(n / bs) bytes."""
+    info = frame_info or FrameInfo()
+    bs = 64 << 10 if info.block_size == BlockSize.Auto else info.block_size.get_size()
+    return 27 * nframes + max_in_bytes + 8 * (-(-max_in_bytes // bs) + nframes)
+
+
+def compress_frames_device_async(d_in, offsets, lengths, out, frame_info: FrameInfo | None = None,
+                                 max_blocks: int | None = None, max_in_bytes: int | None = None,
+                                 ctx: _block.Context | None = None, stream: int | None = None) -> CompressedFrames:
+    """compress_frames_device() without synchronising the host (lz4b200_frame_compress_batch_device_async): the work,
+    the planning of every frame included, is enqueued on torch's current stream (or `stream`) and the call returns at
+    once, so it can be captured in a CUDA graph (torch.cuda.graph).  Every frame inside capacity is byte-identical to
+    what compress_frames_device() writes for it, at the same place in `out`; see CompressedFrames for the result.
+
+    `out` is required (sizing it would need the lengths on the host; compress_out_cap() gives a size that fits any
+    batch within the capacity).  offsets and lengths may be int64 sequences, copied on the call's stream, but under graph
+    capture they must already be int64 CUDA tensors (a copy from host memory cannot be captured); a replay reads them,
+    and d_in, where they are then.
+
+    Frame i is compressed only if frames 0..i together hold at most max_blocks blocks and max_in_bytes input bytes, and
+    their lz4b200_frame_bound sum fits out.numel().  A frame past that writes nothing, has frame_offsets[i] ==
+    frame_offsets[i + 1] == the end of the frames before it, and its status says which limit it passed; the caller can
+    hand those frames to compress_frames_device().  The defaults, max_in_bytes = d_in.numel() and max_blocks =
+    default_compress_max_blocks(d_in.numel(), nframes), hold every batch whose inputs do not overlap in d_in.  Inputs
+    that overlap (the same bytes compressed twice) can pass them, and the frames past them are left out as above.  The
+    scratch (lz4b200_frame_compress_batch_device_async_scratch bytes: about 1.1 bytes per byte of max_in_bytes and 60 per
+    block of capacity) is allocated with torch.empty, so under capture it comes from the graph's pool."""
+    info = frame_info or FrameInfo()
+    if info.block_mode == BlockMode.Linked:
+        raise LinkedBlocksUnsupported()
+    return _compress_frames_async(_native.lib().lz4b200_frame_compress_batch_device_async, d_in, offsets, lengths, out,
+                                  info, max_blocks, max_in_bytes, ctx, stream)
+
+
+def compress_linked_frames_device_async(d_in, offsets, lengths, out, frame_info: FrameInfo | None = None,
+                                        max_blocks: int | None = None, max_in_bytes: int | None = None,
+                                        ctx: _block.Context | None = None,
+                                        stream: int | None = None) -> CompressedFrames:
+    """compress_frames_device_async() for BlockMode::Linked (lz4b200_frame_compress_linked_batch_device_async): frame i
+    is byte-identical to what compress_linked_frames_device() writes for it.  frame_info must have
+    block_mode=BlockMode.Linked (None: the default FrameInfo with linked blocks); an independent one raises ValueError.
+    The chains start in frame order rather than longest first, which changes the time, not the bytes."""
+    info = frame_info or FrameInfo(block_mode=BlockMode.Linked)
+    if info.block_mode != BlockMode.Linked:
+        raise ValueError("compress_linked_frames_device_async: frame_info.block_mode must be BlockMode.Linked")
+    return _compress_frames_async(_native.lib().lz4b200_frame_compress_linked_batch_device_async, d_in, offsets,
+                                  lengths, out, info, max_blocks, max_in_bytes, ctx, stream)
+
+
+def _compress_frames_async(fn, d_in, offsets, lengths, out, info: FrameInfo, max_blocks, max_in_bytes, ctx, stream):
+    import torch
+    _device_u8(d_in, "d_in")
+    _device_u8(out, "out")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    L = _native.lib()
+    with torch.cuda.stream(torch.cuda.ExternalStream(s, device=dev)):
+        # everything on the call's stream, as in decompress_frames_device_async()
+        offs, lens = _device_i64(offsets, dev, "offsets"), _device_i64(lengths, dev, "lengths")
+        n = offs.numel()
+        if lens.numel() != n:
+            raise ValueError("offsets and lengths differ in length")
+        if max_in_bytes is None:
+            max_in_bytes = d_in.numel()
+        if max_blocks is None:
+            max_blocks = default_compress_max_blocks(d_in.numel(), n)
+        if max_blocks < 0 or max_in_bytes < 0:
+            raise ValueError("max_blocks and max_in_bytes must not be negative")
+        nbytes = L.lz4b200_frame_compress_batch_device_async_scratch(ctx.handle, n, max_blocks, max_in_bytes)
+        if nbytes == C.c_size_t(-1).value:
+            raise ValueError("nframes, max_blocks or max_in_bytes is too large")
+        frame_offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        statuses = torch.empty(n, dtype=torch.int32, device=dev)
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    ci = info.to_c()
+    st = fn(ctx.handle, d_in.data_ptr() if d_in.numel() else None, offs.data_ptr(), lens.data_ptr(), C.byref(ci),
+            out.data_ptr(), out.numel(), frame_offsets.data_ptr(), statuses.data_ptr(), n, max_blocks, max_in_bytes,
+            scratch.data_ptr(), nbytes, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return CompressedFrames(out, frame_offsets, statuses)
+
+
 _CONTENT_CHECKSUM = 108
 
 
