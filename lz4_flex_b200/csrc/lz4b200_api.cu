@@ -2216,67 +2216,14 @@ lz4b200_status lz4b200_decompress_batch_host_with_dict(lz4b200_ctx *ctx, const u
 
 // ---- single-block host entry points -----------------------------------------------------------
 
-lz4b200_status lz4b200_compress_into(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
-                                     size_t *written)
-{
-    if (!ctx || !written || (!in && n) || n > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
-    *written = 0;
-    if (cap < lz4b200_max_output_size(n)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;     // compress.rs:338-340
-    uint64_t in_off = 0, out_off = 0;
-    uint32_t in_len = (uint32_t)n, out_len = 0;
-    int32_t status = 0;
-    static const uint8_t zero = 0;
-    lz4b200_status st = lz4b200_compress_batch_host(ctx, n ? in : &zero, &in_off, &in_len, nullptr, out, cap, &out_off,
-                                                    &out_len, &status, 1);
-    if (st != LZ4B200_OK) return st;
-    if (status != LZ4B200_OK) return (lz4b200_status)status;
-    *written = out_len;
-    return LZ4B200_OK;
-}
+}  // extern "C"
 
-lz4b200_status lz4b200_compress_prepend_size(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
-                                             size_t *written)
-{
-    if (!written) return LZ4B200_INVALID_ARGUMENT;
-    *written = 0;
-    if (cap < 4) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
-    wr32(out, (uint32_t)n);                                                              // compress.rs:633/649
-    size_t w = 0;
-    lz4b200_status st = lz4b200_compress_into(ctx, in, n, out + 4, cap - 4, &w);
-    if (st == LZ4B200_OK) *written = w + 4;
-    return st;
-}
+namespace {
 
-lz4b200_status lz4b200_decompress_into(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
-                                       size_t *written, size_t *err_expected, size_t *err_actual)
-{
-    if (!ctx || !written || n > 0xffffffffull || cap > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
-    *written = 0;
-    if (err_expected) *err_expected = 0;
-    if (err_actual) *err_actual = 0;
-    if (n == 0) return LZ4B200_DEC_EXPECTED_ANOTHER_BYTE;                                // decompress.rs:207-209
-    uint64_t in_off = 0, out_off = 0, expected = 0;
-    uint32_t in_len = (uint32_t)n, out_cap = (uint32_t)cap, out_len = 0;
-    int32_t status = 0;
-    uint8_t dummy = 0;
-    lz4b200_status st = lz4b200_decompress_batch_host(ctx, in, &in_off, &in_len, cap ? out : &dummy, &out_off, &out_cap,
-                                                      &out_len, &status, &expected, 1);
-    if (st != LZ4B200_OK) return st;
-    if (status != LZ4B200_OK) {
-        if (status == LZ4B200_DEC_OUTPUT_TOO_SMALL) {
-            if (err_expected) *err_expected = (size_t)expected;
-            if (err_actual) *err_actual = cap;
-        }
-        return (lz4b200_status)status;
-    }
-    *written = out_len;
-    return LZ4B200_OK;
-}
-
-// ---- external dictionary (compress.rs:610-616, 685-693; decompress.rs:462-468, 478-528) ------------------
-
-lz4b200_status lz4b200_compress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict,
-                                               size_t dict_len, uint8_t *out, size_t cap, size_t *written)
+// One block through the host batch pipeline, with the parse flag byte *flag (null: 0) and the external dictionary
+// dict[0, dict_len) (compress.rs:610-616, 685-693).
+lz4b200_status compress_one(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *flag, const uint8_t *dict,
+                            size_t dict_len, uint8_t *out, size_t cap, size_t *written)
 {
     if (!ctx || !written || (!in && n) || n > 0xffffffffull || (!dict && dict_len)) return LZ4B200_INVALID_ARGUMENT;
     *written = 0;
@@ -2285,7 +2232,7 @@ lz4b200_status lz4b200_compress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *
     uint32_t in_len = (uint32_t)n, out_len = 0;
     int32_t status = 0;
     static const uint8_t zero = 0;
-    lz4b200_status st = compress_batch_host_impl(ctx, n ? in : &zero, &in_off, &in_len, nullptr, dict, dict_len, out, cap,
+    lz4b200_status st = compress_batch_host_impl(ctx, n ? in : &zero, &in_off, &in_len, flag, dict, dict_len, out, cap,
                                                  &out_off, &out_len, &status, 1);
     if (st != LZ4B200_OK) return st;
     if (status != LZ4B200_OK) return (lz4b200_status)status;
@@ -2293,48 +2240,24 @@ lz4b200_status lz4b200_compress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *
     return LZ4B200_OK;
 }
 
-// block::compress_into_with_table (compress.rs:744-766).  The reusable CompressTable only decides which table
-// layout / hash the parse uses: Small = u16 entries + 4-byte hash (inputs < 65 535 bytes), Large = u32 entries +
-// 5-byte hash for any size; a Small table handed an input >= 65 535 bytes is upgraded to Large and stays Large.
-// *table_kind carries that state (LZ4B200_TABLE_SMALL / LZ4B200_TABLE_LARGE); the table's memory lives on the GPU.
-lz4b200_status lz4b200_compress_into_with_table(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
-                                                size_t *written, int *table_kind)
-{
-    if (!ctx || !written || !table_kind || (!in && n) || n > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
-    if (*table_kind != LZ4B200_TABLE_SMALL && *table_kind != LZ4B200_TABLE_LARGE) return LZ4B200_INVALID_ARGUMENT;
-    *written = 0;
-    if (n >= 65535 && *table_kind == LZ4B200_TABLE_SMALL) *table_kind = LZ4B200_TABLE_LARGE;      // compress.rs:750-752
-    if (cap < lz4b200_max_output_size(n)) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;                // compress.rs:338-340
-    uint64_t in_off = 0, out_off = 0;
-    uint32_t in_len = (uint32_t)n, out_len = 0;
-    int32_t status = 0;
-    const uint8_t flag = *table_kind == LZ4B200_TABLE_LARGE ? (uint8_t)LZ4B200_BLOCK_HASH5_ALWAYS : (uint8_t)0;
-    static const uint8_t zero = 0;
-    lz4b200_status st = compress_batch_host_impl(ctx, n ? in : &zero, &in_off, &in_len, &flag, nullptr, 0, out, cap,
-                                                 &out_off, &out_len, &status, 1);
-    if (st != LZ4B200_OK) return st;
-    if (status != LZ4B200_OK) return (lz4b200_status)status;
-    *written = out_len;
-    return LZ4B200_OK;
-}
-
-lz4b200_status lz4b200_compress_prepend_size_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n,
-                                                       const uint8_t *dict, size_t dict_len, uint8_t *out, size_t cap,
-                                                       size_t *written)
+// compress_one after the block's length as 4 little-endian bytes.
+lz4b200_status compress_prepend_one(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict, size_t dict_len,
+                                    uint8_t *out, size_t cap, size_t *written)
 {
     if (!written) return LZ4B200_INVALID_ARGUMENT;
     *written = 0;
     if (cap < 4) return LZ4B200_COMPRESS_OUTPUT_TOO_SMALL;
-    wr32(out, (uint32_t)n);
+    wr32(out, (uint32_t)n);                                                              // compress.rs:633/649
     size_t w = 0;
-    lz4b200_status st = lz4b200_compress_into_with_dict(ctx, in, n, dict, dict_len, out + 4, cap - 4, &w);
+    lz4b200_status st = compress_one(ctx, in, n, nullptr, dict, dict_len, out + 4, cap - 4, &w);
     if (st == LZ4B200_OK) *written = w + 4;
     return st;
 }
 
-lz4b200_status lz4b200_decompress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict,
-                                                 size_t dict_len, uint8_t *out, size_t cap, size_t *written,
-                                                 size_t *err_expected, size_t *err_actual)
+// One block through the host batch pipeline, with the external dictionary dict[0, dict_len) (decompress.rs:462-468,
+// 478-528).
+lz4b200_status decompress_one(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict, size_t dict_len,
+                              uint8_t *out, size_t cap, size_t *written, size_t *err_expected, size_t *err_actual)
 {
     if (!ctx || !written || n > 0xffffffffull || cap > 0xffffffffull || (!dict && dict_len)) return LZ4B200_INVALID_ARGUMENT;
     *written = 0;
@@ -2359,18 +2282,81 @@ lz4b200_status lz4b200_decompress_into_with_dict(lz4b200_ctx *ctx, const uint8_t
     return LZ4B200_OK;
 }
 
-lz4b200_status lz4b200_decompress_size_prepended_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n,
-                                                           const uint8_t *dict, size_t dict_len, uint8_t *out,
-                                                           size_t cap, size_t *written, size_t *err_expected,
-                                                           size_t *err_actual)
+// decompress_one of the block after its 4-byte length, into exactly that many bytes of out.
+lz4b200_status decompress_prepended_one(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict,
+                                        size_t dict_len, uint8_t *out, size_t cap, size_t *written,
+                                        size_t *err_expected, size_t *err_actual)
 {
     size_t want = 0;
     if (written) *written = 0;
     lz4b200_status st = lz4b200_uncompressed_size(in, n, &want);
     if (st != LZ4B200_OK) return st;
     if (cap < want) return LZ4B200_INVALID_ARGUMENT;
-    return lz4b200_decompress_into_with_dict(ctx, in + 4, n - 4, dict, dict_len, out, want, written, err_expected,
-                                             err_actual);
+    return decompress_one(ctx, in + 4, n - 4, dict, dict_len, out, want, written, err_expected, err_actual);
+}
+
+}  // namespace
+
+extern "C" {
+
+lz4b200_status lz4b200_compress_into(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
+                                     size_t *written)
+{
+    return compress_one(ctx, in, n, nullptr, nullptr, 0, out, cap, written);
+}
+
+lz4b200_status lz4b200_compress_prepend_size(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
+                                             size_t *written)
+{
+    return compress_prepend_one(ctx, in, n, nullptr, 0, out, cap, written);
+}
+
+lz4b200_status lz4b200_decompress_into(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
+                                       size_t *written, size_t *err_expected, size_t *err_actual)
+{
+    return decompress_one(ctx, in, n, nullptr, 0, out, cap, written, err_expected, err_actual);
+}
+
+lz4b200_status lz4b200_compress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict,
+                                               size_t dict_len, uint8_t *out, size_t cap, size_t *written)
+{
+    return compress_one(ctx, in, n, nullptr, dict, dict_len, out, cap, written);
+}
+
+// block::compress_into_with_table (compress.rs:744-766).  The reusable CompressTable only decides which table
+// layout / hash the parse uses: Small = u16 entries + 4-byte hash (inputs < 65 535 bytes), Large = u32 entries +
+// 5-byte hash for any size; a Small table handed an input >= 65 535 bytes is upgraded to Large and stays Large.
+// *table_kind carries that state (LZ4B200_TABLE_SMALL / LZ4B200_TABLE_LARGE); the table's memory lives on the GPU.
+lz4b200_status lz4b200_compress_into_with_table(lz4b200_ctx *ctx, const uint8_t *in, size_t n, uint8_t *out, size_t cap,
+                                                size_t *written, int *table_kind)
+{
+    if (!ctx || !written || !table_kind || (!in && n) || n > 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
+    if (*table_kind != LZ4B200_TABLE_SMALL && *table_kind != LZ4B200_TABLE_LARGE) return LZ4B200_INVALID_ARGUMENT;
+    if (n >= 65535 && *table_kind == LZ4B200_TABLE_SMALL) *table_kind = LZ4B200_TABLE_LARGE;      // compress.rs:750-752
+    const uint8_t flag = *table_kind == LZ4B200_TABLE_LARGE ? (uint8_t)LZ4B200_BLOCK_HASH5_ALWAYS : (uint8_t)0;
+    return compress_one(ctx, in, n, &flag, nullptr, 0, out, cap, written);
+}
+
+lz4b200_status lz4b200_compress_prepend_size_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n,
+                                                       const uint8_t *dict, size_t dict_len, uint8_t *out, size_t cap,
+                                                       size_t *written)
+{
+    return compress_prepend_one(ctx, in, n, dict, dict_len, out, cap, written);
+}
+
+lz4b200_status lz4b200_decompress_into_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n, const uint8_t *dict,
+                                                 size_t dict_len, uint8_t *out, size_t cap, size_t *written,
+                                                 size_t *err_expected, size_t *err_actual)
+{
+    return decompress_one(ctx, in, n, dict, dict_len, out, cap, written, err_expected, err_actual);
+}
+
+lz4b200_status lz4b200_decompress_size_prepended_with_dict(lz4b200_ctx *ctx, const uint8_t *in, size_t n,
+                                                           const uint8_t *dict, size_t dict_len, uint8_t *out,
+                                                           size_t cap, size_t *written, size_t *err_expected,
+                                                           size_t *err_actual)
+{
+    return decompress_prepended_one(ctx, in, n, dict, dict_len, out, cap, written, err_expected, err_actual);
 }
 
 lz4b200_status lz4b200_uncompressed_size(const uint8_t *in, size_t n, size_t *size)
@@ -2385,12 +2371,7 @@ lz4b200_status lz4b200_decompress_size_prepended(lz4b200_ctx *ctx, const uint8_t
                                                  size_t cap, size_t *written, size_t *err_expected,
                                                  size_t *err_actual)
 {
-    size_t want = 0;
-    if (written) *written = 0;
-    lz4b200_status st = lz4b200_uncompressed_size(in, n, &want);
-    if (st != LZ4B200_OK) return st;
-    if (cap < want) return LZ4B200_INVALID_ARGUMENT;
-    return lz4b200_decompress_into(ctx, in + 4, n - 4, out, want, written, err_expected, err_actual);
+    return decompress_prepended_one(ctx, in, n, nullptr, 0, out, cap, written, err_expected, err_actual);
 }
 
 // ---- frame format ---------------------------------------------------------------------------------
@@ -2506,6 +2487,18 @@ lz4b200_status enqueue_frames(lz4b200_ctx *ctx, const FrameBufs &m, const uint8_
     return LZ4B200_OK;
 }
 
+// The per-block arrays of nb blocks that every synchronous frame encoder fills, from the context's buffers.
+lz4b200_status reserve_frame_blocks(lz4b200_ctx *ctx, uint32_t nb)
+{
+    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
+    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve((size_t)nb + 1));
+    return LZ4B200_OK;
+}
+
 // The pipeline of every synchronous frame encoder: enqueues the n >= 1 frames of plan (placed by fb::plan_frame) on
 // `s` through enqueue_frames, over the context's buffers.  One plan reaches the device as a kernel argument, more with
 // one copy from pageable memory, which cudaMemcpyAsync stages before it returns, so back-to-back calls never share a
@@ -2520,12 +2513,8 @@ lz4b200_status compress_frames(lz4b200_ctx *ctx, const uint8_t *d_in, const fb::
     const uint32_t nb = last.first_block + (uint32_t)fb::frame_blocks(last);
     CTX_CUDA(ctx, ctx->d_fplan.reserve(n));
     CTX_CUDA(ctx, ctx->d_slots.reserve(last.slot_base + fb::frame_slot_bytes(last) + 16));
-    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve((size_t)nb + 1));
+    const lz4b200_status st = reserve_frame_blocks(ctx, nb);
+    if (st != LZ4B200_OK) return st;
     CTX_CUDA(ctx, ctx->d_gdst.reserve(nb));
     if (content_checksum) CTX_CUDA(ctx, ctx->d_content.reserve(n));
     if (n == 1) {
@@ -2569,12 +2558,8 @@ lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_i
     }
     const size_t slot = (lz4b200_max_output_size(block_size) + 15) & ~size_t(15);
     CTX_CUDA(ctx, ctx->d_slots.reserve(slot * nb + 16));
-    CTX_CUDA(ctx, ctx->d_in_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_in_len.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_off.reserve(nb)); CTX_CUDA(ctx, ctx->d_out_cap.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_out_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_status.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_flags.reserve(nb)); CTX_CUDA(ctx, ctx->d_pick.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_info.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_size.reserve(nb));
-    CTX_CUDA(ctx, ctx->d_payload_len.reserve(nb)); CTX_CUDA(ctx, ctx->d_seg_off.reserve(nb + 1));
+    lz4b200_status st = reserve_frame_blocks(ctx, nb);
+    if (st != LZ4B200_OK) return st;
 
     make_uniform_desc_kernel<<<(nb + 255) / 256, 256, 0, s>>>(in_len, (uint32_t)block_size, slot, first_block,
                                                              fb::fresh_period(block_size), nb, ctx->d_in_off.p,
@@ -2583,7 +2568,7 @@ lz4b200_status lz4b200_frame_range_compress(lz4b200_ctx *ctx, const uint8_t *d_i
     CTX_CUDA(ctx, cudaGetLastError());
     BatchArgs a{d_in, ctx->d_in_off.p, ctx->d_in_len.p, ctx->d_flags.p, ctx->d_slots.p, ctx->d_out_off.p,
                 ctx->d_out_cap.p, ctx->d_out_len.p, ctx->d_status.p, nullptr, nb, nullptr};
-    lz4b200_status st = launch_compress(ctx, a, (uint32_t)std::min<size_t>(block_size, in_len), s);
+    st = launch_compress(ctx, a, (uint32_t)std::min<size_t>(block_size, in_len), s);
     if (st != LZ4B200_OK) return st;
     frame_block_info_kernel<<<(nb + 255) / 256, 256, 0, s>>>(ctx->d_out_len.p, ctx->d_in_len.p, nb, 0, ctx->d_info.p,
                                                             ctx->d_pick.p, ctx->d_seg_size.p, ctx->d_payload_len.p);
@@ -2827,21 +2812,29 @@ size_t async_slot_bytes(size_t cap, size_t in_bytes)
     return in_bytes / 100 * 110 + in_bytes % 100 * 110 / 100 + 35 * cap + 16;
 }
 
-// The caller's scratch of lz4b200_frame_compress_batch_device_async, carved into 256-byte aligned arrays: per frame
-// (n) the plans, the linked order and the content hashes; per block (cap) the pipeline's arrays; the slots; the
-// encoder's global-table region (gtab u16 entries, none for the default shape); the ticket words and the device block
-// count.  With a null base only `bytes` is meaningful.
-struct CompressScratch {
-    FrameBufs m{};
-    uint32_t *nb = nullptr;
+// A caller's scratch at `base`, carved into 256-byte aligned arrays in the order take() is called.  With a null base
+// only `bytes`, the size the arrays need, is meaningful.
+struct ScratchCarver {
+    uintptr_t base;
     size_t bytes = 0;
 
-    CompressScratch(void *base, size_t n, size_t cap, size_t slot_bytes, size_t gtab)
+    template <typename T> void take(T *&p, size_t count)
     {
-        auto take = [&](auto *&p, size_t count) {
-            p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + bytes);
-            bytes += (count * sizeof(*p) + 255) & ~size_t(255);
-        };
+        p = reinterpret_cast<T *>(base + bytes);
+        bytes += (count * sizeof(T) + 255) & ~size_t(255);
+    }
+};
+
+// The caller's scratch of lz4b200_frame_compress_batch_device_async: per frame (n) the plans, the linked order and the
+// content hashes; per block (cap) the pipeline's arrays; the slots; the encoder's global-table region (gtab u16
+// entries, none for the default shape); the ticket words and the device block count.
+struct CompressScratch : ScratchCarver {
+    FrameBufs m{};
+    uint32_t *nb = nullptr;
+
+    CompressScratch(void *base, size_t n, size_t cap, size_t slot_bytes, size_t gtab)
+        : ScratchCarver{reinterpret_cast<uintptr_t>(base)}
+    {
         take(m.plan, n); take(m.order, n); take(m.content, n);
         take(m.in_off, cap); take(m.out_off, cap); take(m.seg_off, cap + 1); take(m.gdst, cap);
         take(m.in_len, cap); take(m.out_cap, cap); take(m.out_len, cap); take(m.info, cap); take(m.seg_size, cap);
@@ -2938,27 +2931,6 @@ namespace {
 constexpr uint32_t kHostWalkChunk = 4096;     // descriptors per frame_walk() call on the host
 constexpr uint32_t kDeviceWalkChunk = 65536;  // descriptors one walk launch records on the device (16 B each)
 
-// The frame at in[0, n) in host memory: header and BlockInfo chain.
-void walk_frame_host(const uint8_t *in, size_t n, fw::FrameWalk &w, std::vector<fw::FrameBlockDesc> &blocks)
-{
-    w = fw::FrameWalk{};
-    blocks.clear();
-    while (w.stage != fw::kWalkDone) {
-        const size_t at = blocks.size();
-        blocks.resize(at + kHostWalkChunk);
-        blocks.resize(at + fw::frame_walk(in, n, w, blocks.data() + at, kHostWalkChunk));
-    }
-}
-
-// The block checksum step on the host: the first recorded block whose stored checksum is wrong, or kNoBlock.
-uint32_t first_bad_block_host(const uint8_t *in, const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks)
-{
-    if (!(w.flg & 0x10)) return fw::kNoBlock;
-    for (size_t k = 0; k < blocks.size(); k++)
-        if (!fw::block_checksum_ok(in, blocks[k])) return (uint32_t)k;
-    return fw::kNoBlock;
-}
-
 // The frame at d_in[0, n) in device memory: the walk runs in one GPU thread, kDeviceWalkChunk blocks per launch; only
 // the walk state and the descriptors (16 B per block) come back to the host.  With `verify`, each launch's blocks have
 // their checksums checked on the device and *bad receives the first failing block (kNoBlock: none).
@@ -2997,6 +2969,33 @@ lz4b200_status walk_frame_device(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t
     return LZ4B200_OK;
 }
 
+// The frame at in[0, n), in host memory or with `device` in device memory: header and BlockInfo chain.  With `verify`
+// the block checksums are checked, and the frame ends at the first block that fails.
+lz4b200_status walk_frame(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, size_t n, bool verify,
+                          fw::FrameWalk &w, std::vector<fw::FrameBlockDesc> &blocks)
+{
+    uint32_t bad = fw::kNoBlock;
+    if (device) {
+        const lz4b200_status st = walk_frame_device(ctx, s, in, n, verify, w, blocks, &bad);
+        if (st != LZ4B200_OK) return st;
+    } else {
+        w = fw::FrameWalk{};
+        blocks.clear();
+        while (w.stage != fw::kWalkDone) {
+            const size_t at = blocks.size();
+            blocks.resize(at + kHostWalkChunk);
+            blocks.resize(at + fw::frame_walk(in, n, w, blocks.data() + at, kHostWalkChunk));
+        }
+        for (size_t k = 0; verify && (w.flg & 0x10) && bad == fw::kNoBlock && k < blocks.size(); k++)
+            if (!fw::block_checksum_ok(in, blocks[k])) bad = (uint32_t)k;
+    }
+    if (bad != fw::kNoBlock) {
+        fw::frame_walk_fail_block(w, blocks[bad], bad);
+        blocks.resize(bad);
+    }
+    return LZ4B200_OK;
+}
+
 // Every concatenated frame of in[0, n) (host or, with `device`, device memory), summed over the blocks each walk records.
 // The header's content_size is NOT used: it is untrusted, and a frame whose real size differs must still be delivered
 // in full before ContentLengthError is reported (frame/decompress.rs:312-321).
@@ -3007,13 +3006,8 @@ lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool d
     std::vector<fw::FrameBlockDesc> blocks;
     size_t ip = 0, total = 0;
     while (ip < n) {
-        if (device) {
-            uint32_t bad;
-            const lz4b200_status st = walk_frame_device(ctx, s, in + ip, n - ip, false, w, blocks, &bad);
-            if (st != LZ4B200_OK) return st;
-        } else {
-            walk_frame_host(in + ip, n - ip, w, blocks);
-        }
+        const lz4b200_status st = walk_frame(ctx, s, device, in + ip, n - ip, false, w, blocks);
+        if (st != LZ4B200_OK) return st;
         for (const fw::FrameBlockDesc &b : blocks)
             total += fw::block_stored(b) ? fw::block_len(b) : (size_t)fw::block_decoded_cap(fw::block_len(b), w.bs);
         if (w.status != LZ4B200_OK || !w.closed) break;
@@ -3194,25 +3188,15 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
 
     fw::FrameWalk w;
     std::vector<fw::FrameBlockDesc> blocks;
-    uint32_t bad = fw::kNoBlock;
-    if (device) {
-        const lz4b200_status st = walk_frame_device(ctx, s, in, n, true, w, blocks, &bad);
-        if (st != LZ4B200_OK) return st;
-    } else {
-        walk_frame_host(in, n, w, blocks);
-        bad = first_bad_block_host(in, w, blocks);
-    }
-    if (bad != fw::kNoBlock) {                               // the frame ends at the first block that fails its checksum
-        fw::frame_walk_fail_block(w, blocks[bad], bad);
-        blocks.resize(bad);
-    }
+    lz4b200_status st = walk_frame(ctx, s, device, in, n, true, w, blocks);
+    if (st != LZ4B200_OK) return st;
     *consumed = w.ip;
     lz4b200_xxh32_state host_content;
     fw::xxh32_reset(host_content, 0);
     if (device) CTX_CUDA(ctx, ctx->d_content.reserve(1));
     lz4b200_frame_result r;
-    const lz4b200_status st = decode_frame_blocks(ctx, s, device, in, out, cap, w, blocks, true, 0,
-                                                  device ? ctx->d_content.p : &host_content, &r, d_result);
+    st = decode_frame_blocks(ctx, s, device, in, out, cap, w, blocks, true, 0, device ? ctx->d_content.p : &host_content,
+                             &r, d_result);
     *written = r.written;
     if (st != LZ4B200_OK) return st;
     if (!device && r.status == LZ4B200_OK && w.closed && w.has_checksum &&
@@ -3222,6 +3206,22 @@ lz4b200_status frame_decompress_next_impl(lz4b200_ctx *ctx, cudaStream_t s, bool
     if (err_expected) *err_expected = r.err_expected;
     if (err_actual) *err_actual = r.err_actual;
     return (lz4b200_status)r.status;
+}
+
+// The count walk of the batch's n frames, one thread per frame, into ctx->d_fwalk, d_fcount and d_fnb; `counts`
+// receives the FrameCounts, read back after a synchronise.
+lz4b200_status count_frames(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, const uint64_t *d_frame_off,
+                            const uint64_t *d_frame_len, uint32_t n, std::vector<fw::FrameCount> &counts)
+{
+    CTX_CUDA(ctx, ctx->d_fwalk.reserve(n)); CTX_CUDA(ctx, ctx->d_fcount.reserve(n));
+    CTX_CUDA(ctx, ctx->d_fnb.reserve(2 * (size_t)n));
+    frame_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ctx->frame_budget,
+                                                       ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_fnb.p);
+    CTX_CUDA(ctx, cudaGetLastError());
+    counts.resize(n);
+    CTX_CUDA(ctx, cudaMemcpyAsync(counts.data(), ctx->d_fcount.p, n * sizeof(fw::FrameCount), cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    return LZ4B200_OK;
 }
 
 // The record walk and block checksums of the batch's frames [f0, f0 + gn), whose blocks frame_count_kernel counted into
@@ -3338,14 +3338,9 @@ lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx, const uin
     DeviceGuard guard(ctx->device);
     cudaStream_t s = (cudaStream_t)stream;
     const uint32_t n = (uint32_t)nframes;
-    CTX_CUDA(ctx, ctx->d_fwalk.reserve(n)); CTX_CUDA(ctx, ctx->d_fcount.reserve(n));
-    CTX_CUDA(ctx, ctx->d_fnb.reserve(2 * (size_t)n));
-    frame_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ctx->frame_budget,
-                                                       ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_fnb.p);
-    CTX_CUDA(ctx, cudaGetLastError());
-    std::vector<fw::FrameCount> counts(n);
-    CTX_CUDA(ctx, cudaMemcpyAsync(counts.data(), ctx->d_fcount.p, n * sizeof(fw::FrameCount), cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    std::vector<fw::FrameCount> counts;
+    lz4b200_status st = count_frames(ctx, s, d_in, d_frame_off, d_frame_len, n, counts);
+    if (st != LZ4B200_OK) return st;
 
     // groups of consecutive one-group frames whose slots fit the budget (a linked frame larger than the budget is a group
     // of its own, as in the group loop); at most kGroupItems frames plus blocks per group bound the descriptor arrays
@@ -3372,7 +3367,7 @@ lz4b200_status lz4b200_frame_decompress_batch_device(lz4b200_ctx *ctx, const uin
         slots += c.slot_total;
         items += 1 + c.nblocks;
     }
-    const lz4b200_status st = flush(n);
+    st = flush(n);
     if (st != LZ4B200_OK) return st;
     if (!solo.empty()) {
         // frames the group loop splits (at least one budget of slots) or with more blocks than a group holds: the
@@ -3492,13 +3487,8 @@ lz4b200_status lz4b200_frame_index_device(lz4b200_ctx *ctx, const uint8_t *d_in,
     cudaStream_t s = (cudaStream_t)stream;
     fw::FrameWalk w;
     std::vector<fw::FrameBlockDesc> blocks;
-    uint32_t bad = fw::kNoBlock;
-    lz4b200_status st = walk_frame_device(ctx, s, d_in, n, d_index != nullptr, w, blocks, &bad);
+    lz4b200_status st = walk_frame(ctx, s, true, d_in, n, d_index != nullptr, w, blocks);
     if (st != LZ4B200_OK) return st;
-    if (bad != fw::kNoBlock) {                               // the frame ends at the first block that fails its checksum
-        fw::frame_walk_fail_block(w, blocks[bad], bad);
-        blocks.resize(bad);
-    }
     *nblocks = blocks.size();
     if (!d_index) return LZ4B200_OK;
     if (max_blocks < blocks.size() || blocks.size() >= 0xffffffffull) return LZ4B200_INVALID_ARGUMENT;
@@ -3543,14 +3533,9 @@ lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t 
     DeviceGuard guard(ctx->device);
     cudaStream_t s = (cudaStream_t)stream;
     const uint32_t n = (uint32_t)nframes;
-    CTX_CUDA(ctx, ctx->d_fwalk.reserve(n)); CTX_CUDA(ctx, ctx->d_fcount.reserve(n));
-    CTX_CUDA(ctx, ctx->d_fnb.reserve(2 * (size_t)n));
-    frame_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(d_in, d_frame_off, d_frame_len, n, ctx->frame_budget,
-                                                       ctx->d_fwalk.p, ctx->d_fcount.p, ctx->d_fnb.p);
-    CTX_CUDA(ctx, cudaGetLastError());
-    std::vector<fw::FrameCount> counts(n);
-    CTX_CUDA(ctx, cudaMemcpyAsync(counts.data(), ctx->d_fcount.p, n * sizeof(fw::FrameCount), cudaMemcpyDeviceToHost, s));
-    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    std::vector<fw::FrameCount> counts;
+    lz4b200_status st = count_frames(ctx, s, d_in, d_frame_off, d_frame_len, n, counts);
+    if (st != LZ4B200_OK) return st;
     std::vector<uint64_t> eoff(n);                            // the exclusive scan of the counts
     uint64_t total = 0;
     for (uint32_t f = 0; f < n; f++) { eoff[f] = total; total += counts[f].nblocks; }
@@ -3589,7 +3574,7 @@ lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t 
         }
         nb += k;
     }
-    lz4b200_status st = flush(n);
+    st = flush(n);
     if (st != LZ4B200_OK) return st;
     if (!solo.empty()) {
         std::vector<uint64_t> off(n), len(n);
@@ -3612,11 +3597,10 @@ lz4b200_status lz4b200_frame_index_batch_device(lz4b200_ctx *ctx, const uint8_t 
 // ---- sync-free batch frame decoder ---------------------------------------------------------------------------------------
 namespace {
 
-// The caller's scratch of lz4b200_frame_decompress_batch_device_async, carved into 256-byte aligned arrays: per frame
-// (n) the count walk, the scans, the GroupFrame, the content hash and the capacity and check flags; per block (cap) the
-// record walk, the sizing, and the decoders' arguments and results; the decoders' ticket words and the block count.
-// With a null base only `bytes` is meaningful.
-struct AsyncScratch {
+// The caller's scratch of lz4b200_frame_decompress_batch_device_async: per frame (n) the count walk, the scans, the
+// GroupFrame, the content hash and the capacity and check flags; per block (cap) the record walk, the sizing, and the
+// decoders' arguments and results; the decoders' ticket words and the block count.
+struct AsyncScratch : ScratchCarver {
     fw::FrameWalk *walks;
     fw::FrameCount *counts;
     uint32_t *nb2, *mis;
@@ -3629,14 +3613,9 @@ struct AsyncScratch {
     int32_t *status;
     uint64_t *expected, *gdst, *in_off;
     uint32_t *tickets, *nb;
-    size_t bytes = 0;
 
-    AsyncScratch(void *base, size_t n, size_t nblocks)
+    AsyncScratch(void *base, size_t n, size_t nblocks) : ScratchCarver{reinterpret_cast<uintptr_t>(base)}
     {
-        auto take = [&](auto *&p, size_t count) {
-            p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(reinterpret_cast<uintptr_t>(base) + bytes);
-            bytes += (count * sizeof(*p) + 255) & ~size_t(255);
-        };
         take(walks, n); take(counts, n); take(nb2, 2 * n); take(mis, n); take(scan, 2 * (n + 1)); take(frames, n);
         take(content, n); take(hash, n); take(over, n);
         take(desc, nblocks); take(bframe, nblocks); take(len, nblocks); take(cap, nblocks); take(reach, nblocks);
