@@ -525,7 +525,9 @@ lz4b200_status lz4b200_frame_decompress_next_device(lz4b200_ctx *ctx, const uint
                                                     uint64_t *err_expected, uint64_t *err_actual, void *stream);
 
 /* lz4b200_frame_decoded_bound for frames in device memory (every concatenated frame; content_size ignored); the walk runs
- * on the GPU on `stream`, which the call synchronises. */
+ * on the GPU on `stream`, which the call synchronises.  The first frame is walked as the one-frame decoder walks it;
+ * the rest is split (lz4b200_frame_split_device, below) and its regions bounded in parallel.  That grows the context's
+ * scratch by about 0.2 bytes per input byte, kept as lz4b200_frame_decompress_device keeps it. */
 lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
                                                   void *stream);
 
@@ -710,6 +712,58 @@ uint64_t lz4b200_ctx_last_range_blocks(const lz4b200_ctx *ctx);
 lz4b200_status lz4b200_frame_decoded_bound_batch_device(lz4b200_ctx *ctx,
     const uint8_t *d_in, const uint64_t *d_frame_off, const uint64_t *d_frame_len,
     uint64_t *d_bound, size_t nframes, void *stream);
+
+/* ---- concatenated frames in DEVICE memory (FrameDecoder reading frames back to back, frame/decompress.rs:109-176) -----
+ * The frame format allows frames back to back: a writer that starts a frame at every flush, `cat a.lz4 b.lz4`, or the
+ * output of lz4b200_frame_compress_batch_device stored without its offsets.  The split finds where each frame starts
+ * on the device, so the many-frame calls above (batch decode, batch index, range reads) can take such data.
+ *
+ * Region i of d_in[0, n) is exactly what the serial loop of lz4b200_frame_decompress_next_device visits: p_0 = 0; when
+ * the header and BlockInfo walk of the frame at p_i (block checksums not verified) ends with status OK before n, the
+ * next region starts where that frame ends; otherwise region i, [p_i, n), is the last.  So the last region is what the
+ * loop sees at that point, errors included (a wrong magic, a skippable frame, a truncated tail, a bad header checksum,
+ * BlockTooBig).  A frame whose walk succeeds but whose decode fails (a checksum, a corrupt block) does not end the
+ * split.  n == 0 has no regions. */
+
+/* Device scratch lz4b200_frame_split_device needs for n input bytes and at most max_candidates candidates: about
+ * n / 64 bytes plus 20 bytes per candidate.  SIZE_MAX when max_candidates passes 2^32 - 4 or n passes 2^45.  Host
+ * arithmetic only. */
+size_t lz4b200_frame_split_device_scratch(size_t n, size_t max_candidates);
+
+/* Splits d_in[0, n) into its frames' regions: region r at d_frame_off[r], d_frame_len[r] bytes, for r < min(R,
+ * max_frames).  d_counts[0] receives the regions written and d_counts[1] the input bytes they cover: the input is split
+ * when d_counts[1] == n, otherwise the caller continues at d_in + d_counts[1].
+ *   - A candidate is a position whose 4 bytes are a frame, legacy or skippable magic.  With at most max_candidates of
+ *     them, each candidate's walk reads at most 64 BlockInfo words in parallel and one CTA follows the chain, walking on
+ *     serially only through frames of more blocks; with more, that CTA walks every frame serially (correct, slower).
+ *     Either way the work stays within 64 x candidates + the blocks of the frames on the chain, whatever the payloads
+ *     hold.
+ *   - No host synchronisation: no device-to-host copy, no allocation, no synchronise, and no state on the context, so
+ *     the call can be captured in a CUDA graph.  Everything is enqueued on `stream`.
+ *   - INVALID_ARGUMENT, before anything is enqueued: a null ctx or d_counts, a null d_in with n > 0, a null d_frame_off
+ *     or d_frame_len with max_frames > 0, a null d_scratch with n > 0, scratch_bytes below
+ *     lz4b200_frame_split_device_scratch(n, max_candidates) or that value SIZE_MAX.
+ * Every array and the scratch are device memory; d_in may have any alignment. */
+lz4b200_status lz4b200_frame_split_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint64_t *d_frame_off,
+                                          uint64_t *d_frame_len, size_t max_frames, uint64_t *d_counts,
+                                          size_t max_candidates, void *d_scratch, size_t scratch_bytes, void *stream);
+
+/* The device counterpart of lz4b200_frame_decompress: every concatenated frame of d_in[0, n), outputs back to back in
+ * d_out[0, cap).  The status, *written, *block_status, *err_expected, *err_actual and d_out[0, *written) equal what
+ * the loop of lz4b200_frame_decompress_next_device gives (each frame at d_in + consumed, into d_out + written with the
+ * room left), the failing frame's error and partial output included.  Bytes of d_out past *written may be written
+ * when a frame fails its content checksum.  The first frame goes through lz4b200_frame_decompress_next_device; when it
+ * does not end the input, the rest is split (lz4b200_frame_split_device), each frame's decoded length comes from
+ * lz4b200_frame_index_batch_device, and lz4b200_frame_decompress_batch_device decodes the frames at the scan of those
+ * lengths.  The number of host synchronisations does not depend on the number of frames below 4 194 304.  Scratch is the
+ * context's.  When the input holds more than one frame the call grows it by the split's scratch (about 0.2 bytes per
+ * input byte: about 0.2 GB for 1 GiB) and per region and block the index, placement and result arrays; the context
+ * keeps that memory for its next calls, counts it in lz4b200_ctx_device_bytes and frees it in lz4b200_ctx_destroy.
+ * Work runs on `stream`, which the call synchronises.  INVALID_ARGUMENT: a null ctx or written, a null d_in
+ * with n > 0, a null d_out with cap > 0. */
+lz4b200_status lz4b200_frame_decompress_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint8_t *d_out,
+                                               size_t cap, size_t *written, int *block_status, uint64_t *err_expected,
+                                               uint64_t *err_actual, void *stream);
 
 /* Streaming frame decoder over DEVICE memory: FrameDecoder (frame/decompress.rs:109-342), which reads a frame one
  * block at a time, for compressed bytes that arrive in HBM chunk by chunk (a GPUDirect Storage reader, a network

@@ -180,6 +180,10 @@ SIGNATURES = {
     "lz4b200_frame_decompress_batch_device_async_scratch": (_sz, [_sz, _sz]),
     "lz4b200_frame_decompress_batch_device_async": (_i32, [_vp] * 8 + [_sz, _sz, _vp, _sz, _vp]),
     "lz4b200_frame_decoded_bound_batch_device": (_i32, [_vp] * 5 + [_sz, _vp]),
+    "lz4b200_frame_split_device_scratch": (_sz, [_sz, _sz]),
+    "lz4b200_frame_split_device": (_i32, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
+    "lz4b200_frame_decompress_device": (_i32, [_vp, _vp, _sz, _vp, _sz, _psz, C.POINTER(C.c_int),
+                                               C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), _vp]),
     "lz4b200_frame_index_device": (_i32, [_vp, _vp, _sz, _vp, _sz, _psz, C.POINTER(FrameIndexInfoC), _vp]),
     "lz4b200_frame_decompress_ranges_device": (_i32, [_vp, _vp, _sz, C.POINTER(FrameIndexInfoC)] + [_vp] * 6 + [_sz, _vp]),
     "lz4b200_frame_index_batch_device": (_i32, [_vp] * 4 + [_sz, _vp, _sz, _psz, _vp, _vp, _vp]),

@@ -20,6 +20,7 @@
 #include "lz4b200_frame_batch.cuh"
 #include "lz4b200_frame_encoder.cuh"
 #include "lz4b200_frame_range.cuh"
+#include "lz4b200_frame_split.cuh"
 #include "lz4b200_frame_walk.cuh"
 #include "lz4b200_kernels.cuh"
 #include "lz4b200_enc_linked.cuh"
@@ -39,7 +40,8 @@ namespace lz4b200 {
 
 // Exclusive scan of sizes[0..n) into offs[0..n], offs[n] = total.  One CTA; n is a block count
 // (<= a few 100k), so a single-CTA chunked scan is far below launch noise.
-__device__ __forceinline__ void scan_sizes(const uint32_t *sizes, uint64_t *offs, uint32_t n)
+template <typename T>
+__device__ __forceinline__ void scan_sizes(const T *sizes, uint64_t *offs, uint32_t n)
 {
     __shared__ uint64_t warp_sums[32];
     __shared__ uint64_t carry;
@@ -83,6 +85,10 @@ __global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint32_t *sizes,
                                                           const uint32_t *n_dev)
 {
     scan_sizes(sizes, offs, min(n, *n_dev));
+}
+__global__ void __launch_bounds__(1024) scan_sizes_kernel(const uint64_t *sizes, uint64_t *offs, uint32_t n)
+{
+    scan_sizes(sizes, offs, n);
 }
 
 // Generic gather: segment b copies len[b] bytes from src_base[sel] + src_off[b] to dst + dst_off[b],
@@ -665,6 +671,102 @@ __global__ void __launch_bounds__(128) frame_bound_kernel(const uint8_t *in, con
     bound[f] = total;
 }
 
+// ---- the frame split (lz4b200_frame_split.cuh), behind lz4b200_frame_split_device -----------------------------------
+// Phase 1: each thread counts the candidates among its kSplitThreadBytes positions; each CTA (a tile) sums them.
+__global__ void __launch_bounds__(256) split_count_kernel(const uint8_t *in, uint64_t n, uint8_t *thread_count,
+                                                          uint32_t *tile_count)
+{
+    __shared__ uint32_t warp[8];
+    const uint64_t t = (uint64_t)blockIdx.x * 256 + threadIdx.x, lo = t * fw::kSplitThreadBytes;
+    const uint32_t k = fw::split_scan(in, n, lo, lo + fw::kSplitThreadBytes, nullptr, 0, 0);
+    thread_count[t] = (uint8_t)k;                                  // at most 16: magics never overlap
+    uint32_t sum = k;
+    for (int d = 16; d; d >>= 1) sum += __shfl_xor_sync(kFull, sum, d);
+    if ((threadIdx.x & 31) == 0) warp[threadIdx.x >> 5] = sum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t total = 0;
+        for (int i = 0; i < 8; i++) total += warp[i];
+        tile_count[blockIdx.x] = total;
+    }
+}
+
+// Phase 1: each thread with candidates writes their positions at its tile's offset plus its place in the tile; only
+// the first max_cand candidates are kept.
+__global__ void __launch_bounds__(256) split_emit_kernel(const uint8_t *in, uint64_t n, const uint8_t *thread_count,
+                                                         const uint64_t *tile_off, uint64_t *pos, uint64_t max_cand)
+{
+    __shared__ uint32_t warp[8];
+    const uint64_t base = tile_off[blockIdx.x];
+    if (base >= max_cand) return;
+    const uint64_t t = (uint64_t)blockIdx.x * 256 + threadIdx.x, lo = t * fw::kSplitThreadBytes;
+    const uint32_t k = thread_count[t];
+    uint32_t x = k;                                                // inclusive scan over the CTA
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(kFull, x, d);
+        if ((threadIdx.x & 31) >= (uint32_t)d) x += y;
+    }
+    if ((threadIdx.x & 31) == 31) warp[threadIdx.x >> 5] = x;
+    __syncthreads();
+    for (uint32_t i = 0; i < (threadIdx.x >> 5); i++) x += warp[i];
+    if (k) fw::split_scan(in, n, lo, lo + fw::kSplitThreadBytes, pos, base + x - k, max_cand);
+}
+
+// Phase 2: one thread per candidate, when they all fit max_cand.
+__global__ void __launch_bounds__(128) split_walk_kernel(const uint8_t *in, uint64_t n, const uint64_t *pos,
+                                                         const uint64_t *total, uint32_t max_cand, uint32_t *next,
+                                                         uint64_t *end)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t c = *total;
+    if (i >= c || c > max_cand) return;
+    uint64_t hops = 0, e = n;
+    next[i] = fw::split_candidate(in, n, pos, (uint32_t)c, i, &e, &hops);
+    end[i] = e;
+}
+
+// Phases 3 and 4: thread 0 follows the chain; the CTA loads each window of successor codes and region ends it asks
+// for.  counts[0] receives the regions written, counts[1] the bytes they cover.
+constexpr uint32_t kSplitWindow = 2048;
+__global__ void __launch_bounds__(256) split_chain_kernel(const uint8_t *in, uint64_t n, const uint64_t *pos,
+                                                          const uint32_t *next, const uint64_t *end,
+                                                          const uint64_t *total, uint64_t max_cand, uint64_t *off,
+                                                          uint64_t *len, uint64_t max_frames, uint64_t *counts)
+{
+    __shared__ uint32_t s_next[kSplitWindow];
+    __shared__ uint64_t s_end[kSplitWindow];
+    __shared__ uint32_t s_need;
+    const uint64_t c_all = *total;
+    const uint32_t c = c_all > max_cand ? 0u : (uint32_t)c_all;
+    fw::SplitChain st;
+    fw::SplitWindow win;
+    win.next = s_next;
+    win.end = s_end;
+    if (threadIdx.x == 0) fw::split_chain_init(st, n, pos, c_all, max_cand);
+    for (;;) {
+        if (threadIdx.x == 0) {
+            uint64_t hops = 0;
+            const uint32_t need = fw::split_chain(in, n, pos, c, st, win, off, len, max_frames, &hops);
+            s_need = st.done ? fw::kSplitNoCand : need;
+        }
+        __syncthreads();
+        const uint32_t lo = s_need;
+        if (lo == fw::kSplitNoCand) break;
+        const uint32_t hi = (uint64_t)lo + kSplitWindow < c ? lo + kSplitWindow : c;
+        for (uint32_t k = lo + threadIdx.x; k < hi; k += blockDim.x) {
+            s_next[k - lo] = next[k];
+            s_end[k - lo] = end[k];
+        }
+        win.lo = lo;
+        win.hi = hi;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        counts[0] = st.regions;
+        counts[1] = st.start;
+    }
+}
+
 // Record walk of the group's frames [f0, f0 + gn), one thread per frame: each frame's descriptors at its base (from the
 // scans of the two block-count classes), its block's frame, and its GroupFrame as one group ending the frame.  The frame
 // index passes no output (frame_out_off, frame_out_cap null: output at 0, unbounded) and no content hash (states null).
@@ -1113,6 +1215,14 @@ struct lz4b200_ctx {
     DevBuf<uint64_t> d_rone;
     DevBuf<lz4b200_frame_index_info> d_iinfo;
     DevBuf<uint32_t> d_rsum;
+    // concatenated frames (lz4b200_frame_decompress_device, _decoded_bound_device): the split's scratch, its regions
+    // and counts; per region its bound and their scan, its index info, output offset and cap, and result; the regions'
+    // block index and entry offsets.  Kept, like the other scratch, for the next call of the same size.
+    DevBuf<uint8_t> d_split;
+    DevBuf<uint64_t> d_soff, d_slen, d_scount, d_sbound, d_sout, d_sentry;
+    DevBuf<lz4b200_frame_index_info> d_sinfo;
+    DevBuf<lz4b200_frame_index_entry> d_sindex;
+    DevBuf<lz4b200_frame_result> d_sres;
     uint64_t last_range_blocks = 0;           // block decodes of the last ranges call (lz4b200_ctx_last_range_blocks)
 
     bool check(cudaError_t e, const char *what)
@@ -2996,20 +3106,28 @@ lz4b200_status walk_frame(lz4b200_ctx *ctx, cudaStream_t s, bool device, const u
     return LZ4B200_OK;
 }
 
-// Every concatenated frame of in[0, n) (host or, with `device`, device memory), summed over the blocks each walk records.
-// The header's content_size is NOT used: it is untrusted, and a frame whose real size differs must still be delivered
-// in full before ContentLengthError is reported (frame/decompress.rs:312-321).
-lz4b200_status frame_decoded_bound_impl(lz4b200_ctx *ctx, cudaStream_t s, bool device, const uint8_t *in, size_t n,
-                                        size_t *bound)
+// The decoded bound of the blocks a walk recorded: per block min(block size, 255 x payload), stored blocks their length.
+size_t blocks_bound(const fw::FrameWalk &w, const std::vector<fw::FrameBlockDesc> &blocks)
+{
+    size_t total = 0;
+    for (const fw::FrameBlockDesc &b : blocks)
+        total += fw::block_stored(b) ? fw::block_len(b) : (size_t)fw::block_decoded_cap(fw::block_len(b), w.bs);
+    return total;
+}
+
+// Every concatenated frame of in[0, n) in host memory, summed over the blocks each walk records, up to and including
+// the first frame whose walk fails or is not closed.  The header's content_size is NOT used: it is untrusted, and a
+// frame whose real size differs must still be delivered in full before ContentLengthError is reported
+// (frame/decompress.rs:312-321).
+lz4b200_status frame_decoded_bound_impl(const uint8_t *in, size_t n, size_t *bound)
 {
     fw::FrameWalk w;
     std::vector<fw::FrameBlockDesc> blocks;
     size_t ip = 0, total = 0;
     while (ip < n) {
-        const lz4b200_status st = walk_frame(ctx, s, device, in + ip, n - ip, false, w, blocks);
+        const lz4b200_status st = walk_frame(nullptr, nullptr, false, in + ip, n - ip, false, w, blocks);
         if (st != LZ4B200_OK) return st;
-        for (const fw::FrameBlockDesc &b : blocks)
-            total += fw::block_stored(b) ? fw::block_len(b) : (size_t)fw::block_decoded_cap(fw::block_len(b), w.bs);
+        total += blocks_bound(w, blocks);
         if (w.status != LZ4B200_OK || !w.closed) break;
         ip += w.ip;
     }
@@ -3279,16 +3397,7 @@ lz4b200_status decode_frame_group(lz4b200_ctx *ctx, cudaStream_t s, const uint8_
 lz4b200_status lz4b200_frame_decoded_bound(const uint8_t *in, size_t n, size_t *bound)
 {
     if (!bound || (!in && n)) return LZ4B200_INVALID_ARGUMENT;
-    return frame_decoded_bound_impl(nullptr, nullptr, false, in, n, bound);
-}
-
-lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
-                                                  void *stream)
-{
-    if (!ctx || !bound || (!d_in && n)) return LZ4B200_INVALID_ARGUMENT;
-    *bound = 0;
-    DeviceGuard guard(ctx->device);
-    return frame_decoded_bound_impl(ctx, (cudaStream_t)stream, true, d_in, n, bound);
+    return frame_decoded_bound_impl(in, n, bound);
 }
 
 void lz4b200_ctx_set_frame_budget(lz4b200_ctx *ctx, size_t bytes)
@@ -3689,6 +3798,212 @@ lz4b200_status lz4b200_frame_decompress_batch_device_async(lz4b200_ctx *ctx, con
     return LZ4B200_OK;
 }
 
+// ---- concatenated frames in device memory: the split, and the decoders over it ------------------------------------------
+namespace {
+
+// The caller's scratch of lz4b200_frame_split_device: per scan thread its candidate count, per tile the count and
+// its scan; per candidate slot its position, region end and successor code.
+struct SplitScratch : ScratchCarver {
+    uint8_t *thread_count;
+    uint32_t *tile_count, *next;
+    uint64_t *tile_off, *pos, *end;
+
+    SplitScratch(void *base, uint64_t ntiles, uint64_t max_cand) : ScratchCarver{reinterpret_cast<uintptr_t>(base)}
+    {
+        take(thread_count, ntiles * 256); take(tile_count, ntiles); take(tile_off, ntiles + 1);
+        take(pos, max_cand); take(end, max_cand); take(next, max_cand);
+    }
+};
+
+uint64_t split_tiles(size_t n) { return n / fw::kSplitTile + (n % fw::kSplitTile != 0); }
+
+// The four phases of the split, enqueued on s (lz4b200_frame_split.cuh).
+lz4b200_status enqueue_split(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, size_t n, uint64_t *d_off,
+                             uint64_t *d_len, size_t max_frames, uint64_t *d_counts, size_t max_cand, void *scratch)
+{
+    if (n == 0) {
+        CTX_CUDA(ctx, cudaMemsetAsync(d_counts, 0, 2 * sizeof(uint64_t), s));
+        return LZ4B200_OK;
+    }
+    const uint32_t ntiles = (uint32_t)split_tiles(n);
+    SplitScratch m(scratch, ntiles, max_cand);
+    split_count_kernel<<<ntiles, 256, 0, s>>>(d_in, n, m.thread_count, m.tile_count);
+    scan_sizes_kernel<<<1, 1024, 0, s>>>(m.tile_count, m.tile_off, ntiles);
+    split_emit_kernel<<<ntiles, 256, 0, s>>>(d_in, n, m.thread_count, m.tile_off, m.pos, max_cand);
+    if (max_cand)
+        split_walk_kernel<<<(uint32_t)((max_cand + 127) / 128), 128, 0, s>>>(d_in, n, m.pos, m.tile_off + ntiles,
+                                                                            (uint32_t)max_cand, m.next, m.end);
+    split_chain_kernel<<<1, 256, 0, s>>>(d_in, n, m.pos, m.next, m.end, m.tile_off + ntiles, max_cand, d_off, d_len,
+                                         max_frames, d_counts);
+    CTX_CUDA(ctx, cudaGetLastError());
+    return LZ4B200_OK;
+}
+
+// Regions one split of the decoders below writes at most, and the candidates it keeps: the Python default,
+// 20 bytes per 128 input bytes, which frames that average 128 bytes or more never pass.
+constexpr size_t kSplitChunkFrames = 1u << 22;
+size_t split_default_candidates(size_t n) { return std::min<size_t>(n / 128 + 1024, fw::kSplitMaxCandidates); }
+
+// Splits d_in[0, n) (n > 0) into the context's region arrays ctx->d_soff and d_slen and reads back the region count
+// and the bytes the regions cover.
+lz4b200_status split_regions(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, size_t n, uint64_t *regions,
+                             uint64_t *covered)
+{
+    const size_t cand = split_default_candidates(n), frames = std::min<size_t>(cand + 1, kSplitChunkFrames);
+    const size_t need = lz4b200_frame_split_device_scratch(n, cand);
+    if (need == SIZE_MAX) return LZ4B200_INVALID_ARGUMENT;
+    CTX_CUDA(ctx, ctx->d_split.reserve(need)); CTX_CUDA(ctx, ctx->d_scount.reserve(2));
+    CTX_CUDA(ctx, ctx->d_soff.reserve(frames)); CTX_CUDA(ctx, ctx->d_slen.reserve(frames));
+    const lz4b200_status st = enqueue_split(ctx, s, d_in, n, ctx->d_soff.p, ctx->d_slen.p, frames, ctx->d_scount.p, cand,
+                                            ctx->d_split.p);
+    if (st != LZ4B200_OK) return st;
+    uint64_t h[2];
+    CTX_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_scount.p, sizeof h, cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    *regions = h[0];
+    *covered = h[1];
+    return LZ4B200_OK;
+}
+
+// The frames of the R regions at ctx->d_soff / d_slen over d_in, decoded into d_out from *written on, as the serial
+// loop decodes them: each region's decoded length from the batch index, output offsets from their scan (exact while
+// every earlier frame succeeds), then the batch decoder over the frames up to the first that the index already shows
+// failing or not fitting `cap`.  *written grows by what the frames deliver and *used by the input they consume, up to
+// and including the first frame whose result is not OK, which *r receives (r->status OK: none failed).
+lz4b200_status decode_regions(lz4b200_ctx *ctx, cudaStream_t s, const uint8_t *d_in, uint32_t R, uint8_t *d_out,
+                              size_t cap, size_t *written, size_t *used, lz4b200_frame_result *r)
+{
+    void *stream = (void *)s;
+    size_t entries = 0;
+    lz4b200_status st = lz4b200_frame_index_batch_device(ctx, d_in, ctx->d_soff.p, ctx->d_slen.p, R, nullptr, 0, &entries,
+                                                         nullptr, nullptr, stream);
+    if (st != LZ4B200_OK) return st;
+    CTX_CUDA(ctx, ctx->d_sindex.reserve(std::max<size_t>(entries, 1))); CTX_CUDA(ctx, ctx->d_sentry.reserve(R));
+    CTX_CUDA(ctx, ctx->d_sinfo.reserve(R));
+    st = lz4b200_frame_index_batch_device(ctx, d_in, ctx->d_soff.p, ctx->d_slen.p, R, ctx->d_sindex.p, entries, &entries,
+                                          ctx->d_sentry.p, ctx->d_sinfo.p, stream);
+    if (st != LZ4B200_OK) return st;
+    std::vector<lz4b200_frame_index_info> info(R);
+    CTX_CUDA(ctx, cudaMemcpyAsync(info.data(), ctx->d_sinfo.p, R * sizeof info[0], cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    std::vector<uint64_t> place;                               // output offsets, then caps
+    uint64_t at = *written;
+    for (uint32_t f = 0; f < R; f++) {
+        place.push_back(std::min<uint64_t>(at, cap));
+        if (info[f].result.status != LZ4B200_OK || info[f].content_len > cap - place.back()) break;
+        at += info[f].content_len;
+    }
+    const uint32_t nf = (uint32_t)place.size();
+    for (uint32_t f = 0; f < nf; f++) place.push_back(cap - place[f]);
+    CTX_CUDA(ctx, ctx->d_sout.reserve(2 * (size_t)nf)); CTX_CUDA(ctx, ctx->d_sres.reserve(nf));
+    CTX_CUDA(ctx, cudaMemcpyAsync(ctx->d_sout.p, place.data(), 2 * nf * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    st = lz4b200_frame_decompress_batch_device(ctx, d_in, ctx->d_soff.p, ctx->d_slen.p, d_out, ctx->d_sout.p,
+                                               ctx->d_sout.p + nf, ctx->d_sres.p, nf, stream);
+    if (st != LZ4B200_OK) return st;
+    std::vector<lz4b200_frame_result> res(nf);
+    CTX_CUDA(ctx, cudaMemcpyAsync(res.data(), ctx->d_sres.p, nf * sizeof res[0], cudaMemcpyDeviceToHost, s));
+    CTX_CUDA(ctx, cudaStreamSynchronize(s));
+    *r = lz4b200_frame_result{};
+    for (const lz4b200_frame_result &x : res) {
+        *written += x.written;
+        *used += x.consumed;
+        *r = x;
+        if (x.status != LZ4B200_OK) break;
+    }
+    return LZ4B200_OK;
+}
+
+}  // namespace
+
+size_t lz4b200_frame_split_device_scratch(size_t n, size_t max_candidates)
+{
+    const uint64_t ntiles = split_tiles(n);
+    if (ntiles > 0x7fffffffull || max_candidates > fw::kSplitMaxCandidates) return SIZE_MAX;
+    return SplitScratch(nullptr, ntiles, max_candidates).bytes;
+}
+
+lz4b200_status lz4b200_frame_split_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint64_t *d_frame_off,
+                                          uint64_t *d_frame_len, size_t max_frames, uint64_t *d_counts,
+                                          size_t max_candidates, void *d_scratch, size_t scratch_bytes, void *stream)
+{
+    if (!ctx || !d_counts || (!d_in && n) || (max_frames && (!d_frame_off || !d_frame_len))) return LZ4B200_INVALID_ARGUMENT;
+    const size_t need = lz4b200_frame_split_device_scratch(n, max_candidates);
+    if (need == SIZE_MAX || scratch_bytes < need || (n && !d_scratch)) return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    return enqueue_split(ctx, (cudaStream_t)stream, d_in, n, d_frame_off, d_frame_len, max_frames, d_counts,
+                         max_candidates, d_scratch);
+}
+
+// The first frame as the one-frame device call decodes it; when it does not end the input, the rest split into regions
+// and decoded by decode_regions, a split's worth at a time.
+lz4b200_status lz4b200_frame_decompress_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, uint8_t *d_out,
+                                               size_t cap, size_t *written, int *block_status, uint64_t *err_expected,
+                                               uint64_t *err_actual, void *stream)
+{
+    if (!ctx || !written || (!d_in && n) || (!d_out && cap)) return LZ4B200_INVALID_ARGUMENT;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    size_t ip = 0;
+    lz4b200_status st = lz4b200_frame_decompress_next_device(ctx, d_in, n, d_out, cap, &ip, written, block_status,
+                                                             err_expected, err_actual, stream);
+    if (st != LZ4B200_OK || ip == 0) return st;
+    while (ip < n) {
+        uint64_t R = 0, covered = 0;
+        st = split_regions(ctx, s, d_in + ip, n - ip, &R, &covered);
+        if (st != LZ4B200_OK) return st;
+        size_t used = 0;
+        lz4b200_frame_result r;
+        st = decode_regions(ctx, s, d_in + ip, (uint32_t)R, d_out, cap, written, &used, &r);
+        if (st != LZ4B200_OK) return st;
+        if (r.status != LZ4B200_OK) {
+            if (block_status) *block_status = r.block_status;
+            if (err_expected) *err_expected = r.err_expected;
+            if (err_actual) *err_actual = r.err_actual;
+            return (lz4b200_status)r.status;
+        }
+        if (used == 0) break;
+        ip += used;
+    }
+    return LZ4B200_OK;
+}
+
+// The first frame walked as the one-frame decoder walks it; when it does not end the input, the rest split into
+// regions, each region's bound from frame_bound_kernel and their sum from scan_sizes_kernel, a split's worth at a time.
+lz4b200_status lz4b200_frame_decoded_bound_device(lz4b200_ctx *ctx, const uint8_t *d_in, size_t n, size_t *bound,
+                                                  void *stream)
+{
+    if (!ctx || !bound || (!d_in && n)) return LZ4B200_INVALID_ARGUMENT;
+    *bound = 0;
+    if (n == 0) return LZ4B200_OK;
+    DeviceGuard guard(ctx->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    fw::FrameWalk w;
+    std::vector<fw::FrameBlockDesc> blocks;
+    lz4b200_status st = walk_frame(ctx, s, true, d_in, n, false, w, blocks);
+    if (st != LZ4B200_OK) return st;
+    size_t total = blocks_bound(w, blocks);
+    if (w.status == LZ4B200_OK && w.closed) {
+        for (size_t ip = w.ip; ip < n;) {
+            uint64_t R = 0, covered = 0;
+            st = split_regions(ctx, s, d_in + ip, n - ip, &R, &covered);
+            if (st != LZ4B200_OK) return st;
+            CTX_CUDA(ctx, ctx->d_sbound.reserve(2 * R + 1));
+            frame_bound_kernel<<<(uint32_t)((R + 127) / 128), 128, 0, s>>>(d_in + ip, ctx->d_soff.p, ctx->d_slen.p,
+                                                                          (uint32_t)R, ctx->d_sbound.p);
+            scan_sizes_kernel<<<1, 1024, 0, s>>>((const uint64_t *)ctx->d_sbound.p, ctx->d_sbound.p + R, (uint32_t)R);
+            CTX_CUDA(ctx, cudaGetLastError());
+            uint64_t sum = 0;
+            CTX_CUDA(ctx, cudaMemcpyAsync(&sum, ctx->d_sbound.p + 2 * R, sizeof sum, cudaMemcpyDeviceToHost, s));
+            CTX_CUDA(ctx, cudaStreamSynchronize(s));
+            total += sum;
+            if (covered == 0) break;
+            ip += covered;
+        }
+    }
+    *bound = total;
+    return LZ4B200_OK;
+}
+
 namespace {
 
 constexpr uint32_t kRangeChunk = 65536;                      // ranges planned per launch
@@ -4008,6 +4323,8 @@ size_t lz4b200_ctx_device_bytes(const lz4b200_ctx *ctx)
     add(ctx->d_forder); add(ctx->d_gframe); add(ctx->d_reach); add(ctx->d_rfirst); add(ctx->d_rcount); add(ctx->d_rwant); add(ctx->d_ritem);
     add(ctx->d_rtouch); add(ctx->d_rent); add(ctx->d_rcarry); add(ctx->d_rflag); add(ctx->d_rblk); add(ctx->d_rpiece);
     add(ctx->d_rone); add(ctx->d_iinfo); add(ctx->d_rsum);
+    add(ctx->d_split); add(ctx->d_soff); add(ctx->d_slen); add(ctx->d_scount); add(ctx->d_sbound); add(ctx->d_sout);
+    add(ctx->d_sentry); add(ctx->d_sinfo); add(ctx->d_sindex); add(ctx->d_sres);
     if (const Pipeline *p = ctx->pipe.get()) {
         for (const Lane &l : p->lane) { add(l.in); add(l.slots); add(l.out); }
         add(p->d_tickets);

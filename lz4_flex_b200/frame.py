@@ -318,23 +318,88 @@ def decoded_bound_device(d_in, ctx: _block.Context | None = None, stream: int | 
 def decompress_frame_device(d_in, out=None, ctx: _block.Context | None = None):
     """Every concatenated frame of the device tensor d_in, decoded on the GPU into `out` (a torch CUDA uint8 tensor;
     None: one of lz4b200_frame_decoded_bound_device bytes is allocated).  Returns the view of `out` that holds the
-    decoded bytes.  Raises what decompress_frame() raises for the same bytes."""
+    decoded bytes.  Raises what decompress_frame() raises for the same bytes.  Runs lz4b200_frame_decompress_device:
+    the frames after the first are found with the split (split_frames_device) and decoded in one batch, so the host
+    waits on the GPU a fixed number of times however many frames d_in holds.  When a frame fails its content checksum,
+    the frames after it may have been decoded into `out` past the returned view: only the view is defined.  A d_in of
+    several frames grows the context's device scratch by about 0.2 bytes per input byte, which the context keeps for
+    its next calls (block.Context.close() frees it)."""
     import torch
     _device_u8(d_in, "d_in")
     ctx = ctx or _block.default_context()
     if out is None:
         out = torch.empty(max(decoded_bound_device(d_in, ctx), 1), dtype=torch.uint8, device=d_in.device)
     _device_u8(out, "out")
-    pos, total = 0, 0
-    while pos < d_in.numel():
-        used, w, err = decompress_next_frame_device(d_in[pos:], out[total:], ctx)
-        total += w
-        if err is not None:
-            raise err
-        if used == 0:
-            break
-        pos += used
-    return out[:total]
+    s = torch.cuda.current_stream(d_in.device).cuda_stream
+    n, cap = d_in.numel(), out.numel()
+    w, bs = C.c_size_t(0), C.c_int(0)
+    e1, e2 = C.c_uint64(0), C.c_uint64(0)
+    st = _native.lib().lz4b200_frame_decompress_device(
+        ctx.handle, d_in.data_ptr() if n else None, n, out.data_ptr() if cap else None, cap, C.byref(w), C.byref(bs),
+        C.byref(e1), C.byref(e2), s)
+    if st != 0:
+        raise error_from_status(st, bs.value, ctx.last_cuda_error(), e1.value, e2.value)
+    return out[:w.value]
+
+
+def default_max_candidates(in_len: int) -> int:
+    """The candidate slots split_frames_device() takes when none are given: in_len // 128 + 1024, 20 bytes of scratch
+    each, so about 0.16 bytes per input byte.  A candidate is a position whose 4 bytes are a frame magic: one per frame,
+    plus magics that happen to sit inside payloads.  Frames of 128 bytes or more on average never pass it; past it the
+    split stays exact but walks every frame serially."""
+    return in_len // 128 + 1024
+
+
+@dataclass
+class SplitFrames:
+    """What split_frames_device() returns, int64 CUDA tensors valid once the stream has reached the call: region i is
+    d_in[offsets[i]:offsets[i] + lengths[i]] for i < counts[0]; counts[1] is the input bytes those regions cover (all
+    of d_in unless max_frames cut the split short).  Slots past counts[0] hold empty regions (offset 0, length 0), so
+    all of offsets and lengths can go to a batch call whose size is fixed, as in a captured CUDA graph."""
+    offsets: "object"
+    lengths: "object"
+    counts: "object"
+
+
+def split_frames_device(d_in, max_frames: int | None = None, max_candidates: int | None = None,
+                        ctx: _block.Context | None = None, stream: int | None = None) -> SplitFrames:
+    """Where each concatenated frame of the device tensor d_in starts (lz4b200_frame_split_device): exactly the regions
+    the decompress_next_frame_device() loop visits, the last one holding whatever ends it (a wrong magic, a truncated
+    tail, ...).  The regions feed decompress_frames_device(), index_frames_device() and the range reads.
+
+    No host synchronisation: the work is enqueued on torch's current stream (or `stream`) and the call returns at once,
+    so it can be captured in a CUDA graph.  max_candidates defaults to default_max_candidates(d_in.numel()) and
+    max_frames to max_candidates + 1, one region per candidate and one for a last region that starts at none, so the
+    split is whole unless candidates overflow their slots.  The scratch (lz4b200_frame_split_device_scratch bytes) and
+    the result tensors come from torch.empty, so under capture they come from the graph's pool."""
+    import torch
+    _device_u8(d_in, "d_in")
+    ctx = ctx or _block.default_context()
+    dev = d_in.device
+    s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    n = d_in.numel()
+    if max_candidates is None:
+        max_candidates = default_max_candidates(n)
+    if max_frames is None:
+        max_frames = max_candidates + 1
+    if max_candidates < 0 or max_frames < 0:
+        raise ValueError("max_frames and max_candidates must not be negative")
+    L = _native.lib()
+    nbytes = L.lz4b200_frame_split_device_scratch(n, max_candidates)
+    if nbytes == C.c_size_t(-1).value:
+        raise ValueError("max_candidates or the input is too large for the split")
+    with torch.cuda.stream(torch.cuda.ExternalStream(s, device=dev)):
+        offsets = torch.zeros(max_frames, dtype=torch.int64, device=dev)         # unwritten slots: empty regions
+        lengths = torch.zeros(max_frames, dtype=torch.int64, device=dev)
+        counts = torch.empty(2, dtype=torch.int64, device=dev)
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    st = L.lz4b200_frame_split_device(ctx.handle, d_in.data_ptr() if n else None, n,
+                                      offsets.data_ptr() if max_frames else None,
+                                      lengths.data_ptr() if max_frames else None, max_frames, counts.data_ptr(),
+                                      max_candidates, scratch.data_ptr(), nbytes, s)
+    if st != 0:
+        raise error_from_status(st, detail=ctx.last_cuda_error())
+    return SplitFrames(offsets, lengths, counts)
 
 
 def _device_i64(v, device, what: str):
